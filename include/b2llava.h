@@ -35,6 +35,8 @@ enum { B2_DT_BF16 = 0, B2_DT_F16 = 1, B2_DT_F32 = 2 };
 enum { B2_ACT_NONE = 0, B2_ACT_QUICK_GELU = 1, B2_ACT_GELU_ERF = 2, B2_ACT_SWIGLU = 3 };
 /* logits modes for b2_prefill */
 enum { B2_LOGITS_NONE = 0, B2_LOGITS_LAST = 1, B2_LOGITS_ALL = 2 };
+/* element formats of a KV cache (b2_kv_create_ex) */
+enum { B2_KV_BF16 = 0, B2_KV_E4M3 = 1 };
 
 typedef struct b2_model_desc {
     /* CLIP vision tower (transformers CLIPVisionConfig; reference clip_encoder.py:22-27) */
@@ -90,12 +92,26 @@ int b2_model_finalize(b2_model* m);      /* checks every tensor arrived, allocat
 int b2_model_destroy(b2_model* m);
 /* BASELINE configs[4] ("fp8-weight path"): after finalize, quantise the decoder's Linear weights to e4m3 with one
  * fp32 scale per output channel; decode steps at batch >= 7 then run e4m3 x e4m3 wgmma GEMMs (activations quantised
- * per token on the fly, KV cache stays bf16). Prefill and small-batch decode keep the bf16 weights. The reference has no
+ * per token on the fly; the KV cache format is a separate choice, b2_kv_create_ex). Prefill and small-batch decode keep the bf16 weights. The reference has no
  * fp8 path; oracle/fp8_oracle.py defines the arithmetic and the tolerance (tests/test_fp8_gpu.py). Off unless this call is
  * made: it changes the numerics of the decode step (W8A8), so it is never a default. */
 int b2_model_enable_fp8_decode(b2_model* m);
 
 int b2_kv_create(b2_model* m, int max_batch, int max_seq, b2_kv** out); /* KV cache [L][2][B][H][Smax][128] bf16 */
+/* b2_kv_create with the element format chosen per cache; b2_kv_create == kv_dtype B2_KV_BF16. B2_KV_E4M3 stores K and V as e4m3
+ * bytes, [L][B][H][Smax][128], with one fp32 scale per (layer, sample, head, token) for K and one for V, [L][B][H][Smax]: 264
+ * bytes per head-token instead of 512 (Smax is rounded up to a multiple of 4 inside). A row's scale is amax / 448 over its 128
+ * elements (1 for a zero row) and q = e4m3_rn_satfinite(x / scale), the rule of b2_op_quantize_rows_e4m3; K is quantised after
+ * RoPE. Prefill attends over the unquantised bf16 K / V of its own tokens, so its logits are bit-identical to a bf16 cache's;
+ * only what it stores is quantised. Every decode step attends over what is stored, the token it appends included: scores
+ * and softmax in fp32, score = (q . k_q) * k_scale / sqrt(128), o += p * v_scale * v_q. oracle/kv_fp8_oracle.py defines the
+ * arithmetic and the tolerance (tests/test_kv_fp8_gpu.py). It changes the numerics of decode, so it is never a default. Decode
+ * on an e4m3 cache runs the multi-kernel step at every batch size (the batch <= 8 megakernel reads bf16 caches only): at
+ * small batch the cache is a few percent of a step's bytes, so there the format buys capacity, not speed. Works with bf16 and
+ * e4m3 weights, b2_prefill_slots, the streaming calls and continuous batching. Unknown kv_dtype: -1. */
+int b2_kv_create_ex(b2_model* m, int max_batch, int max_seq, int kv_dtype, b2_kv** out);
+int b2_kv_dtype(b2_kv* kv);              /* B2_KV_BF16 | B2_KV_E4M3 */
+int64_t b2_kv_bytes(b2_kv* kv);          /* device bytes of K, V and their scale arrays */
 int b2_kv_reset(b2_kv* kv);
 int b2_kv_destroy(b2_kv* kv);
 int b2_kv_lengths(b2_kv* kv, int32_t* lens_host, int n);  /* current cache length per sample */
@@ -217,6 +233,16 @@ int b2_op_rope_kv_write(void* qkv, void* kcache, void* vcache, int B, int S, int
 int b2_op_decode_attn(const void* qkv, void* kcache, void* vcache, const int32_t* cur_len, void* out, void* scratch,
                       int B, int H, int Smax, int nsplit, float theta, float scale, void* stream);
 int64_t b2_op_decode_attn_scratch_bytes(int B, int H, int nsplit); /* caller zero-fills the scratch once */
+/* b2_op_decode_attn over an e4m3 cache: k8 / v8 [B,H,Smax,128] e4m3 bytes, kscale / vscale [B,H,Smax] fp32, all 16-byte
+ * aligned, Smax % 4 == 0. Appends the quantised row of the new token (bytes and scale) and attends over the stored values. */
+int b2_op_decode_attn_e4m3(const void* qkv, void* k8, void* v8, float* kscale, float* vscale, const int32_t* cur_len, void* out,
+                           void* scratch, int B, int H, int Smax, int nsplit, float theta, float scale, void* stream);
+/* the split-KV factor a decode step uses for this shape and cache format (from the resident CTAs per SM of the kernel it launches) */
+int b2_op_decode_attn_nsplit(int B, int H, int Smax, int kv_dtype);
+/* prefill's cache write of an e4m3 cache: kstage / vstage [B,H,S,128] bf16 (roped K, V of one layer) -> rows t < seq_lens[b]
+ * (device int32 [B], NULL = S) of k8 / v8 [B,H,Smax,128] and kscale / vscale [B,H,Smax]; rows beyond seq_lens[b] are not written */
+int b2_op_kv_quantize_e4m3(const void* kstage, const void* vstage, void* k8, void* v8, float* kscale, float* vscale,
+                           const int32_t* seq_lens, int B, int S, int H, int Smax, void* stream);
 int b2_op_interleave_gate_up(const void* gate, const void* up, void* out, int I, int h, void* stream);
 int b2_op_im2col(const void* pixels, void* out, int B, int img, int patch, int kpad, void* stream);
 /* Image preprocessing on the device (csrc/preprocess.cu): the reference's llava/mm_utils.py:16-44 (`expand2square` +

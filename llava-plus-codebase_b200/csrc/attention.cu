@@ -8,6 +8,10 @@
 //                      the KV-cache write (modeling_llama.py:269-270 cache update).
 //   decode_attn_bf16 : one-token decode: RoPE + cache append + split-KV attention with coalesced 16-byte
 //                      cache reads and an in-kernel last-CTA merge (HBM-bound: reads each K/V row once).
+//   kv_quantize_e4m3 : prefill's roped bf16 K/V staging slab -> e4m3 cache rows + one fp32 scale per head-token.
+//   decode_attn_e4m3 : decode_attn_bf16 over an e4m3 cache (128-byte rows, scales folded into score and p).
+#include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <math.h>
 
 #include <stdlib.h>
@@ -504,6 +508,287 @@ __global__ void __launch_bounds__(DA_THREADS) decode_attn_kernel(DecodeAttnParam
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// e4m3 KV cache. A cache row is one head of one token: 128 e4m3 bytes + one fp32 scale (amax / 448, 1 for a zero row;
+// the rule of quant_fp8.cu over the 128 elements of the row). K is quantised after RoPE.
+// ------------------------------------------------------------------------------------------------
+constexpr float kE4M3Max = 448.0f;
+
+__device__ __forceinline__ uint32_t pack4_e4m3(float a, float b, float c, float d) {
+    const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(a, b), __NV_SATFINITE, __NV_E4M3);
+    const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(c, d), __NV_SATFINITE, __NV_E4M3);
+    return lo | (hi << 16);
+}
+// 4 e4m3 bytes -> 4 floats through the packed e4m3x2 -> f16x2 conversion (exact: every e4m3 value is an f16 value)
+__device__ __forceinline__ void unpack4_e4m3(uint32_t w, float* f) {
+    uint32_t h01, h23;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h01) : "h"(static_cast<unsigned short>(w & 0xffffu)));
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h23) : "h"(static_cast<unsigned short>(w >> 16)));
+    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&h01));
+    const float2 b = __half22float2(*reinterpret_cast<const __half2*>(&h23));
+    f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y;
+}
+__device__ __forceinline__ void unpack16_e4m3(const uint4& u, float (&f)[16]) {
+    unpack4_e4m3(u.x, f); unpack4_e4m3(u.y, f + 4); unpack4_e4m3(u.z, f + 8); unpack4_e4m3(u.w, f + 12);
+}
+
+// Prefill cache write. src [B][H][S][128] bf16 (K and V staging slabs of one layer) -> dst rows [b][h][t < len[b]] of
+// [B][H][Smax][128] bytes and [B][H][Smax] scales. grid (ceil(S / 64), H, B), 256 threads: a half-warp owns one row (16 lanes
+// x 16-byte loads), amax over its 16 lanes, one 8-byte store per lane; 4 rows of K and of V in flight per half-warp.
+constexpr int KQ_TILE = 64;
+
+__global__ void __launch_bounds__(256)
+kv_quantize_e4m3_kernel(const __nv_bfloat16* __restrict__ ksrc, const __nv_bfloat16* __restrict__ vsrc,
+                        uint8_t* __restrict__ k8, uint8_t* __restrict__ v8, float* __restrict__ kscale,
+                        float* __restrict__ vscale, const int32_t* __restrict__ seq_lens, int S, int H, int Smax) {
+    pdl_trigger();
+    pdl_wait();  // the slabs are written by the upstream kernels, seq_lens by an earlier one
+    const int head = blockIdx.y, b = blockIdx.z;
+    const int hw = threadIdx.x >> 4, c = threadIdx.x & 15;
+    const int len = seq_lens != nullptr ? min(seq_lens[b], S) : S;
+    const int t0 = blockIdx.x * KQ_TILE + hw;
+    const size_t src_row0 = ((size_t)b * H + head) * S, dst_row0 = ((size_t)b * H + head) * Smax;
+    uint4 raw[2][4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+        const int t = t0 + u * 16;
+        if (t < len) {
+            raw[0][u] = ld_stream_16(ksrc + (src_row0 + t) * DA_D + c * 8);
+            raw[1][u] = ld_stream_16(vsrc + (src_row0 + t) * DA_D + c * 8);
+        }
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+        const int t = t0 + u * 16;
+        if (t >= len) continue;  // uniform across the half-warp (the shuffles below stay inside it)
+#pragma unroll
+        for (int kv = 0; kv < 2; ++kv) {
+            const uint4 r = raw[kv][u];
+            const float f[8] = {bf16_lo(r.x), bf16_hi(r.x), bf16_lo(r.y), bf16_hi(r.y),
+                                bf16_lo(r.z), bf16_hi(r.z), bf16_lo(r.w), bf16_hi(r.w)};
+            float amax = 0.f;
+#pragma unroll
+            for (int e = 0; e < 8; ++e) amax = fmaxf(amax, fabsf(f[e]));
+            const unsigned mask = 0xffffu << (threadIdx.x & 16);
+#pragma unroll
+            for (int o = 8; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(mask, amax, o));
+            const float inv = amax > 0.f ? kE4M3Max / amax : 1.0f;
+            const uint2 q = make_uint2(pack4_e4m3(f[0] * inv, f[1] * inv, f[2] * inv, f[3] * inv),
+                                       pack4_e4m3(f[4] * inv, f[5] * inv, f[6] * inv, f[7] * inv));
+            *reinterpret_cast<uint2*>((kv == 0 ? k8 : v8) + (dst_row0 + t) * DA_D + c * 8) = q;
+            if (c == 0) (kv == 0 ? kscale : vscale)[dst_row0 + t] = amax > 0.f ? amax / kE4M3Max : 1.0f;
+        }
+    }
+}
+
+// Decode attention over an e4m3 cache: the contract of decode_attn_kernel (grid (nsplit, H, B), fixed grid, RoPE on q and
+// the new k in-kernel, one CTA per (b, head) appends, self-resetting counters, same partial / merge scratch). A row is
+// 128 bytes, so 8 lanes x 16-byte loads cover a key and the CTA's 16 lane groups take 4 consecutive keys each per pass
+// (64 keys per pass); the 4 scales of a group are one 16-byte load. k_scale multiplies the score after the lane
+// reduction and v_scale is folded into p: dequantisation costs one multiply per key. The appended row is quantised
+// first and the step attends over the stored (dequantised) values, like every later step will.
+constexpr int DA8_KEYS = 4;  // consecutive keys per lane group and pass
+
+struct DecodeAttnE4m3Params {
+    const __nv_bfloat16* qkv;
+    uint8_t* k8;
+    uint8_t* v8;
+    float* kscale;
+    float* vscale;
+    const int32_t* cur_len;
+    __nv_bfloat16* out;
+    float* partial;
+    int32_t* counters;
+    int H, Smax, nsplit;
+    float theta, scale_log2;
+};
+
+__global__ void __launch_bounds__(DA_THREADS) decode_attn_e4m3_kernel(DecodeAttnE4m3Params p) {
+    const int split = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int grp = (warp << 2) | (lane >> 3);  // lane group 0..15
+    const int c = lane & 7;                     // 16-element chunk of the head dim
+    pdl_trigger();
+    pdl_wait();                                 // qkv (previous GEMM) and cur_len (previous step) are upstream outputs
+    const int pos = p.cur_len[b];
+    const int total = pos + 1;
+    const int hd = p.H * DA_D;
+
+    __shared__ float s_q[DA_D];
+    __shared__ float s_knew[DA_D];
+    __shared__ __align__(16) uint8_t s_new8[2][DA_D];  // the appended row as stored: k bytes, v bytes
+    __shared__ float s_newscale[2];
+    __shared__ float s_red[2][4];
+    __shared__ float s_m[16], s_l[16];
+    __shared__ float s_o[16][DA_D];
+    __shared__ int s_last;
+
+    // key range of this split; multiples of DA8_KEYS so that a group's scale vector is 16-byte aligned
+    int chunk = (total + p.nsplit - 1) / p.nsplit;
+    chunk = (chunk + DA8_KEYS - 1) / DA8_KEYS * DA8_KEYS;
+    const int k_begin = split * chunk;
+    const int k_end = min(k_begin + chunk, total);
+    const bool owns_new = (pos >= k_begin) && (pos < k_end);
+
+    const __nv_bfloat16* qrow = p.qkv + (size_t)b * 3 * hd + head * DA_D;
+    {   // RoPE on q (every CTA) and on the new k (the CTA that appends it)
+        const __nv_bfloat16* krow = qrow + hd;
+        const int i = tid & 63;
+        float cs, sn;
+        rope_cos_sin(pos, i, DA_D, p.theta, cs, sn);
+        const float q1 = __bfloat162float(qrow[i]), q2 = __bfloat162float(qrow[i + 64]);
+        if (tid < 64) s_q[i] = rope_apply(q1, -q2, cs, sn); else s_q[i + 64] = rope_apply(q2, q1, cs, sn);
+        if (owns_new) {
+            const float k1 = __bfloat162float(krow[i]), k2 = __bfloat162float(krow[i + 64]);
+            if (tid < 64) s_knew[i] = rope_apply(k1, -k2, cs, sn); else s_knew[i + 64] = rope_apply(k2, k1, cs, sn);
+        }
+    }
+    __syncthreads();
+
+    const size_t rbase = ((size_t)b * p.H + head) * p.Smax;  // first row of this (b, head) slab
+    if (owns_new) {
+        // quantise and append the new token's k (roped) and v: thread tid owns element tid of both rows
+        const float kx = s_knew[tid], vx = __bfloat162float(qrow[2 * hd + tid]);
+        const float ka = warp_max(fabsf(kx)), va = warp_max(fabsf(vx));
+        if (lane == 0) { s_red[0][warp] = ka; s_red[1][warp] = va; }
+        __syncthreads();
+        const float kamax = fmaxf(fmaxf(s_red[0][0], s_red[0][1]), fmaxf(s_red[0][2], s_red[0][3]));
+        const float vamax = fmaxf(fmaxf(s_red[1][0], s_red[1][1]), fmaxf(s_red[1][2], s_red[1][3]));
+        const float kinv = kamax > 0.f ? kE4M3Max / kamax : 1.0f, vinv = vamax > 0.f ? kE4M3Max / vamax : 1.0f;
+        const uint8_t kq = (uint8_t)__nv_cvt_float_to_fp8(kx * kinv, __NV_SATFINITE, __NV_E4M3);
+        const uint8_t vq = (uint8_t)__nv_cvt_float_to_fp8(vx * vinv, __NV_SATFINITE, __NV_E4M3);
+        s_new8[0][tid] = kq; s_new8[1][tid] = vq;
+        p.k8[(rbase + pos) * DA_D + tid] = kq;
+        p.v8[(rbase + pos) * DA_D + tid] = vq;
+        if (tid == 0) {
+            const float ks = kamax > 0.f ? kamax / kE4M3Max : 1.0f, vs = vamax > 0.f ? vamax / kE4M3Max : 1.0f;
+            s_newscale[0] = ks; s_newscale[1] = vs;
+            p.kscale[rbase + pos] = ks; p.vscale[rbase + pos] = vs;
+        }
+        __syncthreads();
+    }
+
+    float qreg[16];
+#pragma unroll
+    for (int e = 0; e < 16; ++e) qreg[e] = s_q[c * 16 + e];
+
+    float m_run = -INFINITY, l_run = 0.f;
+    float acc[16];
+#pragma unroll
+    for (int e = 0; e < 16; ++e) acc[e] = 0.f;
+
+    const uint8_t* kb = p.k8 + rbase * DA_D + c * 16;
+    const uint8_t* vb = p.v8 + rbase * DA_D + c * 16;
+
+    // trip count is CTA-uniform: the shuffles below use the full warp mask
+    for (int kbase = k_begin; kbase < k_end; kbase += 16 * DA8_KEYS) {
+        const int k0 = kbase + grp * DA8_KEYS;
+        uint4 kraw[DA8_KEYS], vraw[DA8_KEYS];
+        float4 ks4 = make_float4(0.f, 0.f, 0.f, 0.f), vs4 = ks4;
+        if (k0 < k_end) {  // k0 % 4 == 0 and Smax % 4 == 0: aligned, and k0 + 3 stays inside the slab's Smax scales
+            ks4 = __ldg(reinterpret_cast<const float4*>(p.kscale + rbase + k0));
+            vs4 = __ldg(reinterpret_cast<const float4*>(p.vscale + rbase + k0));
+        }
+#pragma unroll
+        for (int u = 0; u < DA8_KEYS; ++u) {
+            const int key = k0 + u;
+            if (key < k_end && key != pos) {
+                kraw[u] = ld_stream_16(kb + (size_t)key * DA_D);
+                vraw[u] = ld_stream_16(vb + (size_t)key * DA_D);
+            } else {
+                kraw[u] = make_uint4(0, 0, 0, 0);
+                vraw[u] = make_uint4(0, 0, 0, 0);
+            }
+        }
+        float ksc[DA8_KEYS] = {ks4.x, ks4.y, ks4.z, ks4.w}, vsc[DA8_KEYS] = {vs4.x, vs4.y, vs4.z, vs4.w};
+        float sc[DA8_KEYS];
+        float m_new = m_run;
+#pragma unroll
+        for (int u = 0; u < DA8_KEYS; ++u) {
+            const int key = k0 + u;
+            if (key >= k_end) { ksc[u] = 0.f; vsc[u] = 0.f; }  // whatever lies behind the range never reaches p * v_scale
+            if (key == pos && owns_new) {  // the row appended above: bytes and scales from shared memory
+                kraw[u] = *reinterpret_cast<const uint4*>(&s_new8[0][c * 16]);
+                vraw[u] = *reinterpret_cast<const uint4*>(&s_new8[1][c * 16]);
+                ksc[u] = s_newscale[0]; vsc[u] = s_newscale[1];
+            }
+            float kf[16];
+            unpack16_e4m3(kraw[u], kf);
+            float dot = 0.f;
+#pragma unroll
+            for (int e = 0; e < 16; ++e) dot += qreg[e] * kf[e];
+            dot += __shfl_xor_sync(0xffffffffu, dot, 4);
+            dot += __shfl_xor_sync(0xffffffffu, dot, 2);
+            dot += __shfl_xor_sync(0xffffffffu, dot, 1);
+            sc[u] = key < k_end ? dot * ksc[u] * p.scale_log2 : -INFINITY;
+            m_new = fmaxf(m_new, sc[u]);
+        }
+        // one rescale of the accumulators per pass (4 keys)
+        const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
+        const float corr = exp2f(m_run - m_use);  // m_run = -inf -> 0
+        m_run = m_new;
+        l_run *= corr;
+#pragma unroll
+        for (int e = 0; e < 16; ++e) acc[e] *= corr;
+#pragma unroll
+        for (int u = 0; u < DA8_KEYS; ++u) {
+            const float pr = exp2f(sc[u] - m_use);  // invalid key: exp2(-inf) = 0
+            l_run += pr;
+            const float pv = pr * vsc[u];
+            float vf[16];
+            unpack16_e4m3(vraw[u], vf);
+#pragma unroll
+            for (int e = 0; e < 16; ++e) acc[e] += pv * vf[e];
+        }
+    }
+
+    // ---- merge the 16 lane groups of this CTA ----
+    if (c == 0) { s_m[grp] = m_run; s_l[grp] = l_run; }
+#pragma unroll
+    for (int e = 0; e < 16; ++e) s_o[grp][c * 16 + e] = acc[e];
+    __syncthreads();
+    float m_cta = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) m_cta = fmaxf(m_cta, s_m[i]);
+    float l_cta = 0.f, o_cta = 0.f;  // thread tid owns output element tid
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+        const float w = (s_m[i] == -INFINITY) ? 0.f : exp2f(s_m[i] - m_cta);
+        l_cta += s_l[i] * w;
+        o_cta += s_o[i][tid] * w;
+    }
+    const int bh = b * p.H + head;
+    float* part = p.partial + ((size_t)bh * p.nsplit + split) * (DA_D + 2);
+    part[tid] = o_cta;
+    if (tid == 0) { part[DA_D] = m_cta; part[DA_D + 1] = l_cta; }
+
+    // ---- last CTA of this (b, head) merges the splits ----
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) {
+        const int prev = atomicAdd(&p.counters[bh], 1);
+        s_last = (prev == p.nsplit - 1) ? 1 : 0;
+    }
+    __syncthreads();
+    if (s_last) {
+        __threadfence();
+        const float* pb = p.partial + (size_t)bh * p.nsplit * (DA_D + 2);
+        float m_all = -INFINITY;
+#pragma unroll 8
+        for (int s = 0; s < p.nsplit; ++s) m_all = fmaxf(m_all, __ldcg(pb + (size_t)s * (DA_D + 2) + DA_D));
+        float l_all = 0.f, o_all = 0.f;
+#pragma unroll 8
+        for (int s = 0; s < p.nsplit; ++s) {
+            const float ms = __ldcg(pb + (size_t)s * (DA_D + 2) + DA_D);
+            const float w = (ms == -INFINITY) ? 0.f : exp2f(ms - m_all);
+            l_all += __ldcg(pb + (size_t)s * (DA_D + 2) + DA_D + 1) * w;
+            o_all += __ldcg(pb + (size_t)s * (DA_D + 2) + tid) * w;
+        }
+        p.out[(size_t)b * hd + head * DA_D + tid] = __float2bfloat16_rn(o_all / l_all);
+        if (tid == 0) p.counters[bh] = 0;  // self-reset for the next launch
+    }
+}
+
 }  // namespace
 
 int flash_attn_bf16(const FlashArgs& a, cudaStream_t stream) {
@@ -593,6 +878,57 @@ int decode_attn_bf16(const DecodeAttnArgs& a, cudaStream_t stream) {
     p.scale_log2 = a.scale * 1.4426950408889634f;
     dim3 grid(a.nsplit, a.H, a.B);
     B2_CUDA_CHECK(launch_pdl(decode_attn_kernel, grid, dim3(DA_THREADS), 0, stream, p));
+    B2_LAUNCH_CHECK();
+    return 0;
+}
+
+int decode_attn_e4m3_ctas_per_sm() {
+    static int occ = 0;
+    if (occ == 0) {
+        int n = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, decode_attn_e4m3_kernel, DA_THREADS, 0) != cudaSuccess || n < 1) n = 4;
+        occ = n;
+    }
+    return occ;
+}
+
+int decode_attn_e4m3(const DecodeAttnArgs& a, cudaStream_t stream) {
+    B2_CHECK_ARG(a.D == DA_D, "decode_attn_e4m3: head_dim must be 128 (got %d)", a.D);
+    B2_CHECK_ARG(a.nsplit >= 1 && a.B > 0 && a.H > 0, "decode_attn_e4m3: bad launch shape");
+    B2_CHECK_ARG(a.kscale != nullptr && a.vscale != nullptr, "decode_attn_e4m3: null scale array");
+    B2_CHECK_ARG(a.Smax > 0 && a.Smax % DA8_KEYS == 0, "decode_attn_e4m3: Smax must be a multiple of %d (got %d)", DA8_KEYS, a.Smax);
+    B2_CHECK_ARG(((reinterpret_cast<uintptr_t>(a.kcache) | reinterpret_cast<uintptr_t>(a.vcache) |
+                   reinterpret_cast<uintptr_t>(a.kscale) | reinterpret_cast<uintptr_t>(a.vscale)) & 15) == 0,
+                 "decode_attn_e4m3: caches and scales must be 16-byte aligned");
+    DecodeAttnE4m3Params p;
+    p.qkv = reinterpret_cast<const __nv_bfloat16*>(a.qkv);
+    p.k8 = reinterpret_cast<uint8_t*>(a.kcache);
+    p.v8 = reinterpret_cast<uint8_t*>(a.vcache);
+    p.kscale = a.kscale; p.vscale = a.vscale;
+    p.cur_len = a.cur_len;
+    p.out = reinterpret_cast<__nv_bfloat16*>(a.out);
+    p.partial = a.partial;
+    p.counters = a.counters;
+    p.H = a.H; p.Smax = a.Smax; p.nsplit = a.nsplit;
+    p.theta = a.theta;
+    p.scale_log2 = a.scale * 1.4426950408889634f;
+    dim3 grid(a.nsplit, a.H, a.B);
+    B2_CUDA_CHECK(launch_pdl(decode_attn_e4m3_kernel, grid, dim3(DA_THREADS), 0, stream, p));
+    B2_LAUNCH_CHECK();
+    return 0;
+}
+
+int kv_quantize_e4m3(const void* ksrc, const void* vsrc, void* k8, void* v8, float* kscale, float* vscale,
+                     const int32_t* seq_lens, int B, int S, int H, int D, int Smax, cudaStream_t stream) {
+    B2_CHECK_ARG(D == DA_D, "kv_quantize_e4m3: head_dim must be 128 (got %d)", D);
+    B2_CHECK_ARG(B > 0 && H > 0 && S > 0 && S <= Smax, "kv_quantize_e4m3: B=%d H=%d S=%d Smax=%d", B, H, S, Smax);
+    B2_CHECK_ARG(((reinterpret_cast<uintptr_t>(ksrc) | reinterpret_cast<uintptr_t>(vsrc)) & 15) == 0 &&
+                 ((reinterpret_cast<uintptr_t>(k8) | reinterpret_cast<uintptr_t>(v8)) & 7) == 0,
+                 "kv_quantize_e4m3: slabs must be 16-byte and caches 8-byte aligned");
+    dim3 grid((S + KQ_TILE - 1) / KQ_TILE, H, B);
+    B2_CUDA_CHECK(launch_pdl(kv_quantize_e4m3_kernel, grid, dim3(256), 0, stream, reinterpret_cast<const __nv_bfloat16*>(ksrc),
+                             reinterpret_cast<const __nv_bfloat16*>(vsrc), reinterpret_cast<uint8_t*>(k8),
+                             reinterpret_cast<uint8_t*>(v8), kscale, vscale, seq_lens, S, H, Smax));
     B2_LAUNCH_CHECK();
     return 0;
 }

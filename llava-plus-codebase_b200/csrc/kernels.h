@@ -129,7 +129,8 @@ int rope_kv_write(void* qkv, void* kcache, void* vcache, int B, int S, int H, in
 // split-KV attention over cur_len[b]+1 keys; out [B, H*D] bf16.
 struct DecodeAttnArgs {
     const void* qkv = nullptr;
-    void* kcache = nullptr; void* vcache = nullptr;  // layer base, [Bmax, H, Smax, D]
+    void* kcache = nullptr; void* vcache = nullptr;  // layer base, [Bmax, H, Smax, D] (bf16, or e4m3 bytes)
+    float* kscale = nullptr; float* vscale = nullptr;  // e4m3 cache only: layer base, [Bmax, H, Smax] fp32
     const int32_t* cur_len = nullptr;                // device [B]
     void* out = nullptr;
     float* partial = nullptr;                        // workspace [B*H*nsplit*(D+2)] fp32
@@ -139,6 +140,13 @@ struct DecodeAttnArgs {
 };
 int decode_attn_ctas_per_sm();
 int decode_attn_bf16(const DecodeAttnArgs& a, cudaStream_t stream);
+// the same step over an e4m3 cache (rows of 128 bytes + one fp32 scale per row); Smax % 4 == 0
+int decode_attn_e4m3_ctas_per_sm();
+int decode_attn_e4m3(const DecodeAttnArgs& a, cudaStream_t stream);
+// prefill cache write of an e4m3 cache: roped bf16 K / V of one layer, [B, H, S, D] contiguous, -> rows t < seq_lens[b]
+// (device, null = S) of k8 / v8 [B, H, Smax, D] bytes and kscale / vscale [B, H, Smax]
+int kv_quantize_e4m3(const void* ksrc, const void* vsrc, void* k8, void* v8, float* kscale, float* vscale,
+                     const int32_t* seq_lens, int B, int S, int H, int D, int Smax, cudaStream_t stream);
 
 // ---- persistent decode-step megakernel (decode_mega.cu), batch <= 8 ------------------------------------
 struct MegaLayer {

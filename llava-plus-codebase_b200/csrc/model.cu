@@ -113,12 +113,18 @@ struct b2_model {
     // fp8 decode (BASELINE configs[4]): e4m3 lm_head + scales, quantised activation row buffer + per-token scales
     bool fp8_decode = false;
     DevBuf lm_head8, s_head, xq8, xscale;
+    // e4m3 KV caches: one layer of roped bf16 K / V, [B][H][S][128], that prefill attends over before it is quantised into
+    // the cache (allocated with the first e4m3 cache)
+    DevBuf kstage, vstage;
 };
 
 struct b2_kv {
     b2_model* m = nullptr;
     int max_batch = 0, max_seq = 0;
-    DevBuf k, v;  // [L][B][H][Smax][D]
+    int dtype = B2_KV_BF16;
+    int pitch = 0;       // tokens per (layer, sample, head) slab: max_seq, rounded up to a multiple of 4 for an e4m3 cache
+    DevBuf k, v;         // [L][B][H][pitch][D] bf16, or e4m3 bytes
+    DevBuf kscale, vscale;  // e4m3 cache: [L][B][H][pitch] fp32, one scale per stored row
     DevBuf len_dev, tok, step_counter, out_tokens, attn_partial, attn_counters;
     DevBuf sk_partial, sk_counters;  // stream-K workspace of the skinny decode GEMM (batch 9..128)
     std::vector<int32_t> len_host;
@@ -145,7 +151,12 @@ struct b2_kv {
     int stream_B = 0, stream_tag = 0, stream_scheduled = 0;  // streaming generation in progress: tokens scheduled so far
     DevBuf rows_dev;               // RowState[max_batch] (continuous batching)
     std::vector<RowState> rows_host;
-    size_t layer_stride() const { return (size_t)max_batch * m->d.heads * max_seq * m->hd; }
+    bool e4m3() const { return dtype == B2_KV_E4M3; }
+    size_t elem_bytes() const { return e4m3() ? 1 : 2; }
+    size_t layer_rows() const { return (size_t)max_batch * m->d.heads * pitch; }  // = the layer stride of the scale arrays
+    size_t layer_stride() const { return layer_rows() * m->hd; }                  // elements of k / v
+    char* k_layer(int l) const { return k.as<char>() + (size_t)l * layer_stride() * elem_bytes(); }
+    char* v_layer(int l) const { return v.as<char>() + (size_t)l * layer_stride() * elem_bytes(); }
 };
 
 namespace {
@@ -255,13 +266,13 @@ bool use_skinny(const b2_kv* kv, int B) {
     return !(e != nullptr && e[0] == '0');
 }
 
-int decode_nsplit(int B, int H, int max_seq) {
+int decode_nsplit(int B, int H, int max_seq, int ctas_per_sm) {
     // Split-KV factor of the multi-kernel decode step. The kernel is register-limited to `occ` resident CTAs per SM, so one wave
     // is occ*SMs CTAs. Few (batch, head) pairs: fill one wave; otherwise 3 splits (short enough ranges for the tail wave to
     // overlap, few enough partials for the merge to stay cheap).
     const char* e = getenv("B2_DECODE_NSPLIT");
     if (e != nullptr && atoi(e) >= 1) return atoi(e) > 32 ? 32 : atoi(e);
-    const int cap = decode_attn_ctas_per_sm() * num_sms();
+    const int cap = ctas_per_sm * num_sms();
     int n = cap / (B * H);
     if (n < 3) n = 3;
     if (n > 16) n = 16;
@@ -493,7 +504,7 @@ int encode_chunk(b2_model* m, const void* pixels, int n, void* out, cudaStream_t
 int decode_step_launch(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     const b2_model_desc& d = m->d;
     const int h = d.hidden, I = d.inter, H = d.heads, V = d.vocab;
-    const int nsplit = decode_nsplit(B, H, kv->max_seq);
+    const int nsplit = decode_nsplit(B, H, kv->max_seq, kv->e4m3() ? decode_attn_e4m3_ctas_per_sm() : decode_attn_ctas_per_sm());
     B2_TRY(embed_tokens(kv->tok.as<int32_t>(), m->embed.p, m->x.p, B, h, V, m->err_dev, st));
     // batch <= 8: tensor-core GEMV kernels (falls back to the skinny-M wgmma GEMM when the activations do not fit smem)
     // batch 7..128: swap-AB stream-K GEMM (weights streamed once, all SMs busy); otherwise GEMV kernels (B <= 8) or
@@ -519,16 +530,22 @@ int decode_step_launch(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
         }
         DecodeAttnArgs da;
         da.qkv = m->qkv.p;
-        da.kcache = kv->k.as<bf16>() + (size_t)l * kv->layer_stride();
-        da.vcache = kv->v.as<bf16>() + (size_t)l * kv->layer_stride();
+        da.kcache = kv->k_layer(l);
+        da.vcache = kv->v_layer(l);
         da.cur_len = kv->len_dev.as<int32_t>();
         da.out = m->attn.p;
         da.partial = kv->attn_partial.as<float>();
         da.counters = kv->attn_counters.as<int32_t>();
-        da.B = B; da.H = H; da.D = m->hd; da.Smax = kv->max_seq; da.nsplit = nsplit;
+        da.B = B; da.H = H; da.D = m->hd; da.Smax = kv->pitch; da.nsplit = nsplit;
         da.theta = d.rope_theta;
         da.scale = 1.0f / sqrtf((float)m->hd);
-        B2_TRY(decode_attn_bf16(da, st));
+        if (kv->e4m3()) {
+            da.kscale = kv->kscale.as<float>() + (size_t)l * kv->layer_rows();
+            da.vscale = kv->vscale.as<float>() + (size_t)l * kv->layer_rows();
+            B2_TRY(decode_attn_e4m3(da, st));
+        } else {
+            B2_TRY(decode_attn_bf16(da, st));
+        }
         if (f8) {
             B2_TRY(quantize_rows_e4m3(m->attn.p, h, B, h, m->xq8.p, h, m->xscale.as<float>(), st));
             B2_TRY(skinny8(m, kv, L.wo8.p, L.s_o.as<float>(), m->x.p, h, m->x.p, h, 0, B, h, h, ACT_NONE, st));
@@ -605,7 +622,8 @@ int join_stream(b2_kv* kv, cudaStream_t st, cudaStream_t run) {
 }
 
 // run one step, through the cached CUDA graph when possible
-bool use_mega(const b2_model* m, int B) {
+bool use_mega(const b2_model* m, const b2_kv* kv, int B) {
+    if (kv->e4m3()) return false;  // the megakernel reads bf16 caches only: an e4m3 cache takes the multi-kernel step at every batch
     if (!decode_mega_fits(B, m->d.hidden, m->d.inter) || m->d.layers > 48) return false;
     static int flag = -1;
     if (flag < 0) {
@@ -624,7 +642,7 @@ int decode_step_mega(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     const b2_model_desc& d = m->d;
     MegaParams p;
     p.layers = kv->mega_layers.as<MegaLayer>();
-    p.L = d.layers; p.h = d.hidden; p.I = d.inter; p.H = d.heads; p.V = d.vocab; p.B = B; p.Smax = kv->max_seq;
+    p.L = d.layers; p.h = d.hidden; p.I = d.inter; p.H = d.heads; p.V = d.vocab; p.B = B; p.Smax = kv->pitch;
     int ns = (num_sms() * 16) / (B * d.heads);
     p.nsplit = ns < 1 ? 1 : (ns > 64 ? 64 : ns);
     p.embed = m->embed.as<bf16>(); p.final_norm = m->final_norm.as<bf16>(); p.lm_head = m->lm_head.as<bf16>();
@@ -691,7 +709,7 @@ int decode_step_mega(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
 
 int decode_step_run(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     // B <= 8: one persistent cooperative launch per token (no graph needed: launches queue asynchronously)
-    if (use_mega(m, B)) return decode_step_mega(m, kv, B, st);
+    if (use_mega(m, kv, B)) return decode_step_mega(m, kv, B, st);
     if (kv->warm_B != B) {
         // first step for this batch size runs eagerly: sets function attributes, resolves driver entry points
         if (kv->graph) { cudaGraphExecDestroy(kv->graph); kv->graph = nullptr; kv->graph_B = 0; }
@@ -767,7 +785,7 @@ int b2_init(int device) {
 }
 
 const char* b2_last_error(void) { return g_err; }
-int b2_version(void) { return 1; }
+int b2_version(void) { return 2; }
 unsigned long long b2_launch_count(void) { return g_launch_count; }
 
 int b2_model_create(const b2_model_desc* desc, b2_model** out) {
@@ -942,7 +960,8 @@ int b2_model_destroy(b2_model* m) {
     DevBuf* top[] = {&m->patch_w, &m->cls, &m->pos, &m->pre_g, &m->pre_b, &m->p0_w, &m->p0_b, &m->p2_w, &m->p2_b,
                      &m->embed, &m->final_norm, &m->lm_head, &m->v_col, &m->v_patch, &m->v_hidden, &m->v_xn,
                      &m->v_qkv, &m->v_attn, &m->v_mlp, &m->v_feats, &m->p_mid, &m->p_done, &m->enc_pixels, &m->enc_out, &m->x, &m->xn, &m->qkv, &m->attn,
-                     &m->act, &m->last_idx, &m->xlast, &m->logits, &m->splice_idx, &m->lm_head8, &m->s_head, &m->xq8, &m->xscale};
+                     &m->act, &m->last_idx, &m->xlast, &m->logits, &m->splice_idx, &m->lm_head8, &m->s_head, &m->xq8, &m->xscale,
+                     &m->kstage, &m->vstage};
     for (DevBuf* b : top) b->free();
     for (VitLayer& L : m->vit) {
         DevBuf* bs[12] = {&L.ln1_g, &L.ln1_b, &L.wqkv, &L.bqkv, &L.wo, &L.bo, &L.ln2_g, &L.ln2_b, &L.w1, &L.b1, &L.w2, &L.b2};
@@ -989,7 +1008,13 @@ int b2_model_enable_fp8_decode(b2_model* m) {
 }
 
 int b2_kv_create(b2_model* m, int max_batch, int max_seq, b2_kv** out) {
+    return b2_kv_create_ex(m, max_batch, max_seq, B2_KV_BF16, out);
+}
+
+int b2_kv_create_ex(b2_model* m, int max_batch, int max_seq, int kv_dtype, b2_kv** out) {
     B2_CHECK_ARG(m && out, "b2_kv_create: null argument");
+    B2_CHECK_ARG(kv_dtype == B2_KV_BF16 || kv_dtype == B2_KV_E4M3, "b2_kv_create: unknown kv_dtype %d (B2_KV_BF16 = 0, B2_KV_E4M3 = 1)",
+                 kv_dtype);
     B2_CHECK_ARG(max_batch >= 1 && max_batch <= m->d.max_batch, "b2_kv_create: max_batch %d exceeds model max_batch %d",
                  max_batch, m->d.max_batch);
     B2_CHECK_ARG(max_seq >= 1, "b2_kv_create: max_seq must be positive");
@@ -999,9 +1024,21 @@ int b2_kv_create(b2_model* m, int max_batch, int max_seq, b2_kv** out) {
     kv->m = m;
     kv->max_batch = max_batch;
     kv->max_seq = max_seq;
-    const size_t per = (size_t)m->d.layers * kv->layer_stride() * 2;
+    kv->dtype = kv_dtype;
+    kv->pitch = kv->e4m3() ? (max_seq + 3) / 4 * 4 : max_seq;  // decode_attn_e4m3 loads 4 scales as one 16-byte vector
+    const size_t per = (size_t)m->d.layers * kv->layer_stride() * kv->elem_bytes();
+    const size_t per_scale = kv->e4m3() ? (size_t)m->d.layers * kv->layer_rows() * sizeof(float) : 0;
     int r = 0;
+    if (kv->e4m3() && m->kstage.p == nullptr) {
+        const size_t stage = (size_t)m->d.max_batch * m->d.max_seq * m->d.hidden * 2;
+        if ((r = m->kstage.alloc(stage)) != 0 || (r = m->vstage.alloc(stage)) != 0) {
+            m->kstage.free();
+            delete kv;
+            return r;
+        }
+    }
     if ((r = kv->k.alloc(per)) != 0 || (r = kv->v.alloc(per)) != 0 ||
+        (r = kv->kscale.alloc(per_scale)) != 0 || (r = kv->vscale.alloc(per_scale)) != 0 ||
         (r = kv->len_dev.alloc((size_t)max_batch * 4)) != 0 || (r = kv->tok.alloc((size_t)max_batch * 4)) != 0 ||
         (r = kv->step_counter.alloc(4)) != 0) {
         b2_kv_destroy(kv);
@@ -1015,8 +1052,8 @@ int b2_kv_create(b2_model* m, int max_batch, int max_seq, b2_kv** out) {
             LlamaLayer& L = m->ll[l];
             tbl[l].ln1 = L.ln1.as<bf16>(); tbl[l].wqkv = L.wqkv.as<bf16>(); tbl[l].wo = L.wo.as<bf16>();
             tbl[l].ln2 = L.ln2.as<bf16>(); tbl[l].wgu = L.wgu.as<bf16>(); tbl[l].wd = L.wd.as<bf16>();
-            tbl[l].kcache = kv->k.as<bf16>() + (size_t)l * kv->layer_stride();
-            tbl[l].vcache = kv->v.as<bf16>() + (size_t)l * kv->layer_stride();
+            tbl[l].kcache = reinterpret_cast<bf16*>(kv->k_layer(l));  // read by the megakernel, which a bf16 cache alone reaches
+            tbl[l].vcache = reinterpret_cast<bf16*>(kv->v_layer(l));
         }
         if ((r = kv->mega_layers.alloc(tbl.size() * sizeof(MegaLayer))) != 0 || (r = kv->mega_sync.alloc(64)) != 0) {
             b2_kv_destroy(kv);
@@ -1065,6 +1102,7 @@ int b2_kv_create(b2_model* m, int max_batch, int max_seq, b2_kv** out) {
     memset(kv->ring_host, 0, (size_t)kv->ring_cap * max_batch * 4);
     cudaMemset(kv->k.p, 0, per);
     cudaMemset(kv->v.p, 0, per);
+    if (per_scale) { cudaMemset(kv->kscale.p, 0, per_scale); cudaMemset(kv->vscale.p, 0, per_scale); }
     cudaMemset(kv->len_dev.p, 0, (size_t)max_batch * 4);
     cudaMemset(kv->tok.p, 0, (size_t)max_batch * 4);
     cudaMemset(kv->step_counter.p, 0, 4);
@@ -1110,11 +1148,21 @@ int b2_kv_destroy(b2_kv* kv) {
     if (kv->own_stream) cudaStreamDestroy(kv->own_stream);
     if (kv->ev_fork) cudaEventDestroy(kv->ev_fork);
     if (kv->ev_join) cudaEventDestroy(kv->ev_join);
-    DevBuf* bs[] = {&kv->k, &kv->v, &kv->len_dev, &kv->tok, &kv->step_counter, &kv->out_tokens, &kv->attn_partial,
+    DevBuf* bs[] = {&kv->k, &kv->v, &kv->kscale, &kv->vscale, &kv->len_dev, &kv->tok, &kv->step_counter, &kv->out_tokens, &kv->attn_partial,
                     &kv->attn_counters, &kv->mega_layers, &kv->mega_sync, &kv->sk_partial, &kv->sk_counters, &kv->sstate, &kv->rows_dev, &kv->rope_tab};
     for (DevBuf* b : bs) b->free();
     delete kv;
     return 0;
+}
+
+int b2_kv_dtype(b2_kv* kv) {
+    B2_CHECK_ARG(kv != nullptr, "b2_kv_dtype: null");
+    return kv->dtype;
+}
+
+int64_t b2_kv_bytes(b2_kv* kv) {
+    B2_CHECK_ARG(kv != nullptr, "b2_kv_bytes: null");
+    return (int64_t)(kv->k.bytes + kv->v.bytes + kv->kscale.bytes + kv->vscale.bytes);
 }
 
 int b2_kv_lengths(b2_kv* kv, int32_t* lens_host, int n) {
@@ -1243,7 +1291,11 @@ int b2_prefill_slots(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* 
     // lengths / last-row indices travel as kernel parameters: no pinned staging, no stream sync in this call
     B2_TRY(set_i32_pairs(kv->len_dev.as<int32_t>() + slot0, lens.data(), m->last_idx.as<int32_t>(), last.data(), B, st));
     for (int b = 0; b < B; ++b) kv->len_host[slot0 + b] = lens[b];
-    const size_t slot_off = (size_t)slot0 * H * kv->max_seq * m->hd;  // cache slabs of the first slot this call fills
+    const size_t slot_rows = (size_t)slot0 * H * kv->pitch;  // cache rows in front of the first slot this call fills
+    const bool q8 = kv->e4m3();
+    // e4m3 cache: the producers below write one layer of roped bf16 K / V into the staging slab [B][H][S][128] (a cache with
+    // Smax = S), attention reads it there, and kv_quantize_e4m3 then stores the layer's cache rows and scales
+    const int kv_pitch = q8 ? S : kv->pitch;
 
     B2_CUDA_CHECK(cudaMemcpyAsync(m->x.p, embeds, (size_t)T * h * 2, cudaMemcpyDeviceToDevice, st));
     // RoPE + KV write fused into the QKV GEMM where the CTA-pair kernel is the one that runs anyway (M >= 512; 256-column pair
@@ -1252,29 +1304,35 @@ int b2_prefill_slots(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* 
     { const char* e = getenv("B2_ROPE_FUSED"); if (e != nullptr && e[0] == '0') rope_fused = false; }
     for (int l = 0; l < d.layers; ++l) {
         LlamaLayer& L = m->ll[l];
-        bf16* kc = kv->k.as<bf16>() + (size_t)l * kv->layer_stride() + slot_off;
-        bf16* vc = kv->v.as<bf16>() + (size_t)l * kv->layer_stride() + slot_off;
+        bf16* kc = q8 ? m->kstage.as<bf16>() : reinterpret_cast<bf16*>(kv->k_layer(l)) + slot_rows * m->hd;
+        bf16* vc = q8 ? m->vstage.as<bf16>() : reinterpret_cast<bf16*>(kv->v_layer(l)) + slot_rows * m->hd;
         B2_TRY(rmsnorm_bf16(m->x.p, h, L.ln1.p, m->xn.p, T, h, d.rms_eps, st));
         if (rope_fused) {
             // QKV projection with RoPE and the cache write in its epilogue (CTA-pair kernel): q -> qkv buffer, k / v -> cache
             GemmArgs g;
             g.A = m->xn.p; g.lda = h; g.W = L.wqkv.p; g.ldw = h; g.out = m->qkv.p; g.ld_out = 3 * h;
             g.M = T; g.N = 3 * h; g.K = h; g.act = ACT_ROPE_QKV;
-            g.rope.table = kv->rope_tab.p; g.rope.kcache = kc; g.rope.vcache = vc; g.rope.S = S; g.rope.H = H; g.rope.Smax = kv->max_seq;
+            g.rope.table = kv->rope_tab.p; g.rope.kcache = kc; g.rope.vcache = vc; g.rope.S = S; g.rope.H = H; g.rope.Smax = kv_pitch;
             B2_TRY(gemm_bf16_2cta(g, st));
         } else {
             B2_TRY(gemm(m->xn.p, h, L.wqkv.p, h, nullptr, nullptr, 0, m->qkv.p, 3 * h, 0, T, 3 * h, h, ACT_NONE, st));
-            B2_TRY(rope_kv_write(m->qkv.p, kc, vc, B, S, H, m->hd, kv->max_seq, d.rope_theta, st));
+            B2_TRY(rope_kv_write(m->qkv.p, kc, vc, B, S, H, m->hd, kv_pitch, d.rope_theta, st));
         }
         FlashArgs fa;
         fa.q = m->qkv.p; fa.q_bs = (int64_t)S * 3 * h; fa.q_ts = 3 * h; fa.q_hs = m->hd;
-        fa.k = kc; fa.k_bs = (int64_t)H * kv->max_seq * m->hd; fa.k_ts = m->hd; fa.k_hs = (int64_t)kv->max_seq * m->hd;
+        fa.k = kc; fa.k_bs = (int64_t)H * kv_pitch * m->hd; fa.k_ts = m->hd; fa.k_hs = (int64_t)kv_pitch * m->hd;
         fa.v = vc; fa.v_bs = fa.k_bs; fa.v_ts = m->hd; fa.v_hs = fa.k_hs;
         fa.o = m->attn.p; fa.o_bs = (int64_t)S * h; fa.o_ts = h; fa.o_hs = m->hd;
         fa.seq_lens = kv->len_dev.as<int32_t>() + slot0;
         fa.B = B; fa.H = H; fa.S = S; fa.D = m->hd; fa.causal = 1;
         fa.scale = 1.0f / sqrtf((float)m->hd);
         B2_TRY(flash_attn_bf16(fa, st));
+        if (q8) {
+            const size_t row0 = (size_t)l * kv->layer_rows() + slot_rows;
+            B2_TRY(kv_quantize_e4m3(kc, vc, kv->k.as<uint8_t>() + row0 * m->hd, kv->v.as<uint8_t>() + row0 * m->hd,
+                                    kv->kscale.as<float>() + row0, kv->vscale.as<float>() + row0,
+                                    kv->len_dev.as<int32_t>() + slot0, B, S, H, m->hd, kv->pitch, st));
+        }
         B2_TRY(gemm(m->attn.p, h, L.wo.p, h, nullptr, m->x.p, h, m->x.p, h, 0, T, h, h, ACT_NONE, st));
         B2_TRY(rmsnorm_bf16(m->x.p, h, L.ln2.p, m->xn.p, T, h, d.rms_eps, st));
         B2_TRY(gemm(m->xn.p, h, L.wgu.p, h, nullptr, nullptr, 0, m->act.p, I, 0, T, 2 * I, h, ACT_SWIGLU, st));
@@ -1658,6 +1716,29 @@ int b2_op_decode_attn(const void* qkv, void* kcache, void* vcache, const int32_t
     da.partial = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(scratch) + off);
     da.B = B; da.H = H; da.D = 128; da.Smax = Smax; da.nsplit = nsplit; da.theta = theta; da.scale = scale;
     return decode_attn_bf16(da, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2_op_decode_attn_e4m3(const void* qkv, void* k8, void* v8, float* kscale, float* vscale, const int32_t* cur_len, void* out,
+                           void* scratch, int B, int H, int Smax, int nsplit, float theta, float scale, void* stream) {
+    B2_CHECK_ARG(qkv && k8 && v8 && kscale && vscale && cur_len && out && scratch, "b2_op_decode_attn_e4m3: null argument");
+    DecodeAttnArgs da;
+    da.qkv = qkv; da.kcache = k8; da.vcache = v8; da.kscale = kscale; da.vscale = vscale; da.cur_len = cur_len; da.out = out;
+    da.counters = reinterpret_cast<int32_t*>(scratch);
+    da.partial = reinterpret_cast<float*>(reinterpret_cast<char*>(scratch) + (((size_t)B * H * 4 + 255) / 256) * 256);
+    da.B = B; da.H = H; da.D = 128; da.Smax = Smax; da.nsplit = nsplit; da.theta = theta; da.scale = scale;
+    return decode_attn_e4m3(da, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2_op_decode_attn_nsplit(int B, int H, int Smax, int kv_dtype) {
+    B2_CHECK_ARG(B >= 1 && H >= 1 && Smax >= 1, "b2_op_decode_attn_nsplit: bad shape");
+    B2_CHECK_ARG(kv_dtype == B2_KV_BF16 || kv_dtype == B2_KV_E4M3, "b2_op_decode_attn_nsplit: unknown kv_dtype %d", kv_dtype);
+    return decode_nsplit(B, H, Smax, kv_dtype == B2_KV_E4M3 ? decode_attn_e4m3_ctas_per_sm() : decode_attn_ctas_per_sm());
+}
+
+int b2_op_kv_quantize_e4m3(const void* kstage, const void* vstage, void* k8, void* v8, float* kscale, float* vscale,
+                           const int32_t* seq_lens, int B, int S, int H, int Smax, void* stream) {
+    B2_CHECK_ARG(kstage && vstage && k8 && v8 && kscale && vscale, "b2_op_kv_quantize_e4m3: null argument");
+    return kv_quantize_e4m3(kstage, vstage, k8, v8, kscale, vscale, seq_lens, B, S, H, 128, Smax, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int b2_op_interleave_gate_up(const void* gate, const void* up, void* out, int I, int h, void* stream) {

@@ -19,6 +19,8 @@ LIB_PATH = os.environ.get(
 DT_BF16, DT_F16, DT_F32 = 0, 1, 2
 ACT_NONE, ACT_QUICK_GELU, ACT_GELU_ERF, ACT_SWIGLU = 0, 1, 2, 3
 LOGITS_NONE, LOGITS_LAST, LOGITS_ALL = 0, 1, 2
+KV_BF16, KV_E4M3 = 0, 1
+KV_DTYPES = {"bf16": KV_BF16, "e4m3": KV_E4M3}
 INT32_MIN = -(2**31)
 ERR_TOKEN_RANGE, ERR_IMAGE_ROW_RANGE, ERR_SPLICE_SLOTS = 1, 2, 4
 
@@ -70,6 +72,9 @@ SIGNATURES = {
     "b2_model_destroy": (_i32, [_vp]),
     "b2_model_enable_fp8_decode": (_i32, [_vp]),
     "b2_kv_create": (_i32, [_vp, _i32, _i32, _c.POINTER(_vp)]),
+    "b2_kv_create_ex": (_i32, [_vp, _i32, _i32, _i32, _c.POINTER(_vp)]),
+    "b2_kv_dtype": (_i32, [_vp]),
+    "b2_kv_bytes": (_i64, [_vp]),
     "b2_kv_reset": (_i32, [_vp]),
     "b2_kv_destroy": (_i32, [_vp]),
     "b2_kv_lengths": (_i32, [_vp, _c.POINTER(_c.c_int32), _i32]),
@@ -105,6 +110,9 @@ SIGNATURES = {
     "b2_op_rope_kv_write": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp]),
     "b2_op_decode_attn": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _f32, _vp]),
     "b2_op_decode_attn_scratch_bytes": (_i64, [_i32, _i32, _i32]),
+    "b2_op_decode_attn_e4m3": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _f32, _vp]),
+    "b2_op_decode_attn_nsplit": (_i32, [_i32, _i32, _i32, _i32]),
+    "b2_op_kv_quantize_e4m3": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
     "b2_op_interleave_gate_up": (_i32, [_vp, _vp, _vp, _i32, _i32, _vp]),
     "b2_op_im2col": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _vp]),
 }
@@ -168,6 +176,13 @@ def ptr(t):
     return _vp(t.data_ptr())
 
 
+def kv_dtype_code(dtype):
+    """"bf16" | "e4m3" -> B2_KV_*; anything else is a ValueError (before anything is allocated)."""
+    if dtype not in KV_DTYPES:
+        raise ValueError(f"unknown KV cache dtype {dtype!r}: expected one of {sorted(KV_DTYPES)}")
+    return KV_DTYPES[dtype]
+
+
 def launch_count():
     return int(load_library().b2_launch_count())
 
@@ -176,14 +191,21 @@ _TORCH_DT = {torch.bfloat16: DT_BF16, torch.float16: DT_F16, torch.float32: DT_F
 
 
 class KVCache:
-    """Device KV cache handle (b2_kv): [layers][B][heads][max_seq][128] bf16 for K and V."""
+    """Device KV cache handle (b2_kv): [layers][B][heads][max_seq][128] for K and V; bf16, or with dtype="e4m3" one byte per
+    element plus an fp32 scale per (layer, sample, head, token) — 0.516 x the bytes, different decode numerics (b2llava.h)."""
 
-    def __init__(self, engine, max_batch, max_seq):
+    def __init__(self, engine, max_batch, max_seq, dtype="bf16"):
         self.engine = engine
-        self.max_batch, self.max_seq = int(max_batch), int(max_seq)
+        self.max_batch, self.max_seq, self.dtype = int(max_batch), int(max_seq), dtype
+        code = kv_dtype_code(dtype)
         h = _vp()
-        check(engine.lib.b2_kv_create(engine.handle, self.max_batch, self.max_seq, ctypes.byref(h)), "b2_kv_create")
+        check(engine.lib.b2_kv_create_ex(engine.handle, self.max_batch, self.max_seq, code, ctypes.byref(h)), "b2_kv_create_ex")
         self.handle = h
+
+    @property
+    def nbytes(self):
+        """Device bytes of K, V and their scales."""
+        return int(self.engine.lib.b2_kv_bytes(self.handle))
 
     def reset(self):
         check(self.engine.lib.b2_kv_reset(self.handle), "b2_kv_reset")
@@ -250,9 +272,9 @@ class Engine:
         with torch.cuda.device(self.index):
             check(self.lib.b2_model_enable_fp8_decode(self.handle), "b2_model_enable_fp8_decode")
 
-    def new_kv(self, max_batch, max_seq):
+    def new_kv(self, max_batch, max_seq, dtype="bf16"):
         with torch.cuda.device(self.index):
-            kv = KVCache(self, max_batch, max_seq)
+            kv = KVCache(self, max_batch, max_seq, dtype)
         self._kvs.add(kv)
         return kv
 

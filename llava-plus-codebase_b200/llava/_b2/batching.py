@@ -61,13 +61,13 @@ class RequestStream:
 
 
 class ContinuousBatcher:
-    def __init__(self, engine, slots, max_seq, _cuda=None):
-        """`_cuda`: the namespace streams / events come from (torch.cuda; the CPU tests of the scheduling logic pass a stand-in)."""
+    def __init__(self, engine, slots, max_seq, kv_dtype="bf16", _cuda=None):
+        """`kv_dtype`: element format of the shared cache ("bf16" | "e4m3"). `_cuda`: the namespace streams / events come from (torch.cuda; the CPU tests of the scheduling logic pass a stand-in)."""
         self._cuda = _cuda if _cuda is not None else torch.cuda
         if slots < 2:
             raise ValueError("continuous batching needs at least 2 slots")
         self.engine, self.slots, self.max_seq = engine, int(slots), int(max_seq)
-        self.kv = engine.new_kv(self.slots, self.max_seq)
+        self.kv = engine.new_kv(self.slots, self.max_seq) if kv_dtype == "bf16" else engine.new_kv(self.slots, self.max_seq, dtype=kv_dtype)
         self.pending = queue.Queue()
         self.active = {}                      # slot -> Request
         self.free = list(range(self.slots))[::-1]

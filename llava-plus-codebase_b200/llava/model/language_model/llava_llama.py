@@ -24,7 +24,7 @@ from transformers.modeling_outputs import CausalLMOutputWithPast
 
 from ..llava_arch import LlavaMetaModel, LlavaMetaForCausalLM
 from ..multimodal_encoder.clip_encoder import _Holder, _read_checkpoint_dir
-from ..._b2 import Engine, KVCache, LOGITS_ALL, LOGITS_LAST, ERR_SPLICE_SLOTS, last_error, make_sampling
+from ..._b2 import Engine, KVCache, LOGITS_ALL, LOGITS_LAST, ERR_SPLICE_SLOTS, kv_dtype_code, last_error, make_sampling
 
 
 class LlavaConfig(LlamaConfig):
@@ -37,8 +37,8 @@ class _KVPool:
     (llava/serve/model_worker.py:174-185, :230-243), and a shared cache would let request B's prefill overwrite request
     A's context mid-decode. Caches are created on demand (up to `cap`, then acquire() blocks) and reused."""
 
-    def __init__(self, engine, max_batch, max_seq, cap):
-        self.engine, self.max_batch, self.max_seq, self.cap = engine, max_batch, max_seq, max(1, int(cap))
+    def __init__(self, engine, max_batch, max_seq, cap, dtype="bf16"):
+        self.engine, self.max_batch, self.max_seq, self.cap, self.dtype = engine, max_batch, max_seq, max(1, int(cap)), dtype
         self._cond = threading.Condition()
         self._free, self._made = [], 0
 
@@ -50,7 +50,7 @@ class _KVPool:
                 return self._free.pop()
             self._made += 1
         try:
-            return self.engine.new_kv(self.max_batch, self.max_seq)
+            return _new_kv(self.engine, self.max_batch, self.max_seq, self.dtype)
         except Exception:
             with self._cond:
                 self._made -= 1
@@ -61,6 +61,10 @@ class _KVPool:
         with self._cond:
             self._free.append(kv)
             self._cond.notify()
+
+
+def _new_kv(engine, max_batch, max_seq, dtype):
+    return engine.new_kv(max_batch, max_seq) if dtype == "bf16" else engine.new_kv(max_batch, max_seq, dtype=dtype)
 
 
 class PastKeyValues:
@@ -240,6 +244,10 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             raise RuntimeError("LlavaLlamaForCausalLM weights must be on a CUDA (sm_90a) device: model.to('cuda'); "
                                "there is no CPU path")
         c, vc = self.config, vt.config
+        # KV cache format of every cache this model creates: config.b2_kv_dtype or B2_KV_DTYPE ("bf16" default, "e4m3": half the
+        # cache bytes, decode numerics change — include/b2llava.h, b2_kv_create_ex); checked before anything is allocated
+        self._kv_dtype = getattr(c, "b2_kv_dtype", None) or os.environ.get("B2_KV_DTYPE") or "bf16"
+        kv_dtype_code(self._kv_dtype)
         max_seq = self._limits["max_seq"] or min(getattr(c, "max_position_embeddings", 4096), 4096)
         desc = dict(
             image_size=vc.image_size, patch_size=vc.patch_size, vit_hidden=vc.hidden_size,
@@ -264,7 +272,8 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         if getattr(c, "b2_fp8_decode", False) or os.environ.get("B2_FP8_DECODE") == "1":
             eng.enable_fp8_decode()
         self._pool = _KVPool(eng, desc["max_batch"], desc["max_seq"],
-                             getattr(c, "b2_max_concurrent_generations", None) or int(os.environ.get("B2_MAX_GENERATIONS", "8")))
+                             getattr(c, "b2_max_concurrent_generations", None) or int(os.environ.get("B2_MAX_GENERATIONS", "8")),
+                             dtype=self._kv_dtype)
         self._fwd_kvs = []
         self._engine = eng
         return eng
@@ -276,7 +285,7 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         with self._engine_lock:
             if self._batcher is None:
                 from ..._b2.batching import ContinuousBatcher
-                self._batcher = ContinuousBatcher(eng, slots, eng.desc.max_seq)
+                self._batcher = ContinuousBatcher(eng, slots, eng.desc.max_seq, kv_dtype=self._kv_dtype)
             return self._batcher
 
     def _check_limits(self, eng, B, need_seq):
@@ -291,7 +300,7 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         with self._fwd_lock:
             cap = max(1, int(getattr(self.config, "b2_forward_caches", 2)))
             if len(self._fwd_kvs) < cap:
-                kv = eng.new_kv(eng.desc.max_batch, eng.desc.max_seq)
+                kv = _new_kv(eng, eng.desc.max_batch, eng.desc.max_seq, self._kv_dtype)
                 kv._lease_serial = 0
             else:
                 kv = self._fwd_kvs.pop(0)
