@@ -149,7 +149,7 @@ int b2_splice_ids(b2_model* m, const int64_t* input_ids, int B, int Lt, int k_pe
 int b2_async_error(b2_model* m, int* code_out);
 /* LlamaModel.forward prefill over inputs_embeds [B,S,hidden] (HF modeling_llama.py:375-425 and :303-332 per
  * layer), right-padded rows with seq_lens_host[b] valid tokens (NULL => all S). Fills the KV cache from
- * position 0. logits_out: B2_LOGITS_LAST -> fp32 [B,vocab] at each sample's last valid position;
+ * position 0 (b2_prefill_at: from a given position). logits_out: B2_LOGITS_LAST -> fp32 [B,vocab] at each sample's last valid position;
  * B2_LOGITS_ALL -> fp32 [B,S,vocab] (the reference's lm_head over all positions, llava_llama.py:88-99). */
 int b2_prefill(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* seq_lens_host, int B, int S,
                void* logits_out, int logits_mode, void* stream);
@@ -157,6 +157,15 @@ int b2_prefill(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* seq_le
  * a new request is prefilled while the rest of the batch keeps its context). b2_prefill == slot0 0. */
 int b2_prefill_slots(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* seq_lens_host, int B, int S, int slot0,
                      void* logits_out, int logits_mode, void* stream);
+/* Prefill of a chunk appended at a given cache position (multi-turn chat: the turn's new tokens behind the conversation
+ * already in the cache). Sample b's S-row chunk (seq_lens_host[b] valid tokens, NULL => all S) goes to positions
+ * start_host[b] .. start_host[b] + len - 1 of slot slot0 + b: RoPE at those positions, attention over the cache rows
+ * [0, start_host[b]) plus the chunk itself (causal). Needs start_host[b] <= the slot's current length (a smaller start rewinds
+ * the slot) and start_host[b] + len <= max_seq; afterwards the slot's length is start_host[b] + len. logits_out as in
+ * b2_prefill, over the chunk's positions. start_host NULL (or all zeros) is b2_prefill_slots. On an e4m3 cache the chunk
+ * attends over the stored prefix as bf16(q * scale) and its own unquantised K / V, and stores only its own rows. */
+int b2_prefill_at(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* start_host, const int32_t* seq_lens_host, int B,
+                  int S, int slot0, void* logits_out, int logits_mode, void* stream);
 /* One autoregressive step (reference decode branch llava_arch.py:103-112 + HF one-token forward): tokens [B]
  * int32 (host or device) are embedded, run through the decoder against the cache (appending one K/V row per
  * layer), logits_out fp32 [B,vocab] (nullable), next_tokens_out int32 [B] = argmax (nullable, host or device). */
@@ -226,9 +235,18 @@ int b2_op_rmsnorm(const void* x, const void* gamma, void* y, int rows, int cols,
 /* q,k,v,o: [B,S,H,D] bf16 contiguous; seq_lens device int32 [B] or NULL */
 int b2_op_flash_attn(const void* q, const void* k, const void* v, void* o, const int32_t* seq_lens, int B, int S,
                      int H, int D, int causal, float scale, void* stream);
+/* causal attention of a chunk against a KV cache: q, o [B,S,H,128] bf16; kcache/vcache [B,H,Smax,128] bf16; pos0 / seq_lens
+ * device int32 [B] (seq_lens nullable = S). Query row t of sample b sits at position pos0[b] + t and attends cache rows
+ * 0 .. pos0[b] + t; the cache must already hold the chunk's own rows (b2_op_rope_kv_write_at). wgmma kernel only. */
+int b2_op_flash_attn_kv(const void* q, const void* kcache, const void* vcache, void* o, const int32_t* pos0, const int32_t* seq_lens,
+                        int B, int S, int H, int Smax, float scale, void* stream);
 /* qkv [B*S, 3*H*D] (q roped in place); kcache/vcache [B,H,Smax,D] */
 int b2_op_rope_kv_write(void* qkv, void* kcache, void* vcache, int B, int S, int H, int D, int Smax, float theta,
                         void* stream);
+/* b2_op_rope_kv_write for a chunk at cache position pos0[b] (device int32 [B]): row t of sample b is rotated for position
+ * pos0[b] + t and stored at that cache row; rows at or beyond Smax are rotated but not stored */
+int b2_op_rope_kv_write_at(void* qkv, void* kcache, void* vcache, const int32_t* pos0, int B, int S, int H, int D, int Smax,
+                           float theta, void* stream);
 /* qkv [B,3*H*128]; caches [B,H,Smax,128]; cur_len device int32 [B]; out [B,H*128]; scratch from b2_op_decode_attn_scratch */
 int b2_op_decode_attn(const void* qkv, void* kcache, void* vcache, const int32_t* cur_len, void* out, void* scratch,
                       int B, int H, int Smax, int nsplit, float theta, float scale, void* stream);
@@ -243,6 +261,14 @@ int b2_op_decode_attn_nsplit(int B, int H, int Smax, int kv_dtype);
  * (device int32 [B], NULL = S) of k8 / v8 [B,H,Smax,128] and kscale / vscale [B,H,Smax]; rows beyond seq_lens[b] are not written */
 int b2_op_kv_quantize_e4m3(const void* kstage, const void* vstage, void* k8, void* v8, float* kscale, float* vscale,
                            const int32_t* seq_lens, int B, int S, int H, int Smax, void* stream);
+/* b2_op_kv_quantize_e4m3 of a chunk at cache position pos0[b] (device int32 [B]): kstage / vstage [B,H,S_src,128]; chunk row
+ * t < seq_lens[b] (NULL = S) is read from slab row pos0[b] + t and stored at cache row pos0[b] + t; nothing else is written */
+int b2_op_kv_quantize_e4m3_at(const void* kstage, const void* vstage, void* k8, void* v8, float* kscale, float* vscale,
+                              const int32_t* pos0, const int32_t* seq_lens, int B, int S, int S_src, int H, int Smax, void* stream);
+/* the stored prefix of an e4m3 cache as bf16: rows t < pos0[b] (device int32 [B]) of k8 / v8 [B,H,Smax,128] with kscale / vscale
+ * [B,H,Smax] -> kdst / vdst [B,H,S_dst,128] row t = bf16(float(q) * scale); rows >= min(pos0[b], S_dst) are not written */
+int b2_op_kv_dequantize_e4m3(const void* k8, const void* v8, const float* kscale, const float* vscale, const int32_t* pos0,
+                             void* kdst, void* vdst, int B, int H, int Smax, int S_dst, void* stream);
 int b2_op_interleave_gate_up(const void* gate, const void* up, void* out, int I, int h, void* stream);
 int b2_op_im2col(const void* pixels, void* out, int B, int img, int patch, int kpad, void* stream);
 /* Image preprocessing on the device (csrc/preprocess.cu): the reference's llava/mm_utils.py:16-44 (`expand2square` +

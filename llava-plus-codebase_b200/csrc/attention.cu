@@ -277,12 +277,17 @@ __global__ void rope_table_kernel(uint32_t* __restrict__ table, int Smax, int D,
 // = q/k/v elements [c*8, c*8+8) and their rotation partners [D/2 + c*8, ...), six loads and six stores of 16 B.
 __global__ void __launch_bounds__(256)
 rope_kv_write_kernel(__nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ kcache,
-                     __nv_bfloat16* __restrict__ vcache, int S, int H, int D, int Smax, float theta) {
+                     __nv_bfloat16* __restrict__ vcache, const int32_t* __restrict__ pos0, int S, int H, int D, int Smax,
+                     float theta) {
     __shared__ float s_c[128], s_s[128];  // D/2 <= 128
     pdl_trigger();
     pdl_wait();  // inputs are outputs of the upstream kernel (programmatic dependent launch)
     const int row = blockIdx.x;  // b*S + t
-    const int b = row / S, t = row % S;
+    const int b = row / S;
+    // absolute position of the token: its RoPE angle and its cache row. With an offset, padding rows of a chunk may lie
+    // beyond the cache: they are rotated (q stays finite) but not stored.
+    const int t = row % S + (pos0 != nullptr ? pos0[b] : 0);
+    const bool store = t < Smax;
     const int hd = H * D;
     const int half = D / 2;
     for (int i = threadIdx.x; i < half; i += blockDim.x) rope_cos_sin(t, i, D, theta, s_c[i], s_s[i]);
@@ -313,6 +318,7 @@ rope_kv_write_kernel(__nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict_
         }
         *reinterpret_cast<uint4*>(q + o1) = make_uint4(oq1[0], oq1[1], oq1[2], oq1[3]);
         *reinterpret_cast<uint4*>(q + o2) = make_uint4(oq2[0], oq2[1], oq2[2], oq2[3]);
+        if (!store) continue;
         const size_t co = (((size_t)b * H + h) * Smax + t) * D + c * 8;
         *reinterpret_cast<uint4*>(kcache + co) = make_uint4(ok1[0], ok1[1], ok1[2], ok1[3]);
         *reinterpret_cast<uint4*>(kcache + co + half) = make_uint4(ok2[0], ok2[1], ok2[2], ok2[3]);
@@ -540,14 +546,17 @@ constexpr int KQ_TILE = 64;
 __global__ void __launch_bounds__(256)
 kv_quantize_e4m3_kernel(const __nv_bfloat16* __restrict__ ksrc, const __nv_bfloat16* __restrict__ vsrc,
                         uint8_t* __restrict__ k8, uint8_t* __restrict__ v8, float* __restrict__ kscale,
-                        float* __restrict__ vscale, const int32_t* __restrict__ seq_lens, int S, int H, int Smax) {
+                        float* __restrict__ vscale, const int32_t* __restrict__ seq_lens, const int32_t* __restrict__ pos0,
+                        int S, int S_src, int H, int Smax) {
     pdl_trigger();
     pdl_wait();  // the slabs are written by the upstream kernels, seq_lens by an earlier one
     const int head = blockIdx.y, b = blockIdx.z;
     const int hw = threadIdx.x >> 4, c = threadIdx.x & 15;
-    const int len = seq_lens != nullptr ? min(seq_lens[b], S) : S;
+    // chunk rows t < len, stored at row p0 + t of the slab and of the cache (rows outside either are never touched)
+    const int p0 = pos0 != nullptr ? pos0[b] : 0;
+    const int len = min(seq_lens != nullptr ? min(seq_lens[b], S) : S, min(S_src, Smax) - p0);
     const int t0 = blockIdx.x * KQ_TILE + hw;
-    const size_t src_row0 = ((size_t)b * H + head) * S, dst_row0 = ((size_t)b * H + head) * Smax;
+    const size_t src_row0 = ((size_t)b * H + head) * S_src + p0, dst_row0 = ((size_t)b * H + head) * Smax + p0;
     uint4 raw[2][4];
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
@@ -577,6 +586,37 @@ kv_quantize_e4m3_kernel(const __nv_bfloat16* __restrict__ ksrc, const __nv_bfloa
                                        pack4_e4m3(f[4] * inv, f[5] * inv, f[6] * inv, f[7] * inv));
             *reinterpret_cast<uint2*>((kv == 0 ? k8 : v8) + (dst_row0 + t) * DA_D + c * 8) = q;
             if (c == 0) (kv == 0 ? kscale : vscale)[dst_row0 + t] = amax > 0.f ? amax / kE4M3Max : 1.0f;
+        }
+    }
+}
+
+// The stored prefix of a cache as bf16, for a prefill chunk that attends over it: rows t < pos0[b] of k8 / v8 [B][H][Smax][128]
+// -> bf16(float(q) * scale) at row t of dst [B][H][S_dst][128]. grid (ceil(S_dst / 64), H, B), 256 threads: 16 lanes per
+// row, 8 bytes in and 16 bytes out per lane.
+__global__ void __launch_bounds__(256)
+kv_dequantize_e4m3_kernel(const uint8_t* __restrict__ k8, const uint8_t* __restrict__ v8, const float* __restrict__ kscale,
+                          const float* __restrict__ vscale, const int32_t* __restrict__ pos0, __nv_bfloat16* __restrict__ kdst,
+                          __nv_bfloat16* __restrict__ vdst, int H, int Smax, int S_dst) {
+    pdl_trigger();
+    pdl_wait();
+    const int head = blockIdx.y, b = blockIdx.z;
+    const int hw = threadIdx.x >> 4, c = threadIdx.x & 15;
+    const int n = min(pos0[b], min(Smax, S_dst));
+    const size_t src_row0 = ((size_t)b * H + head) * Smax, dst_row0 = ((size_t)b * H + head) * S_dst;
+#pragma unroll
+    for (int u = 0; u < KQ_TILE / 16; ++u) {
+        const int t = blockIdx.x * KQ_TILE + hw + u * 16;
+        if (t >= n) break;
+#pragma unroll
+        for (int kv = 0; kv < 2; ++kv) {
+            const uint2 q = *reinterpret_cast<const uint2*>((kv == 0 ? k8 : v8) + (src_row0 + t) * DA_D + c * 8);
+            const float sc = (kv == 0 ? kscale : vscale)[src_row0 + t];
+            float f[8];
+            unpack4_e4m3(q.x, f);
+            unpack4_e4m3(q.y, f + 4);
+            *reinterpret_cast<uint4*>((kv == 0 ? kdst : vdst) + (dst_row0 + t) * DA_D + c * 8) =
+                make_uint4(pack_bf16(f[0] * sc, f[1] * sc), pack_bf16(f[2] * sc, f[3] * sc),
+                           pack_bf16(f[4] * sc, f[5] * sc), pack_bf16(f[6] * sc, f[7] * sc));
         }
     }
 }
@@ -797,6 +837,7 @@ int flash_attn_bf16(const FlashArgs& a, cudaStream_t stream) {
     // wgmma kernel unless B2_FLASH_TC=0 selects the mma.sync one (A/B knob, re-read per call: scripts/attn_bench.py)
     const char* e = getenv("B2_FLASH_TC");
     const bool use_tc = e == nullptr || e[0] != '0';
+    B2_CHECK_ARG(use_tc || a.pos0 == nullptr, "flash_attn: queries at a cache offset need the wgmma kernel (B2_FLASH_TC=0 is set)");
     return use_tc ? flash_attn_tc_bf16(a, stream) : flash_attn_mma_bf16(a, stream);
 }
 
@@ -840,13 +881,13 @@ int rope_table_build(void* table, int Smax, int D, float theta, cudaStream_t str
 }
 
 int rope_kv_write(void* qkv, void* kcache, void* vcache, int B, int S, int H, int D, int Smax, float theta,
-                  cudaStream_t stream) {
-    B2_CHECK_ARG(S <= Smax, "rope_kv_write: S=%d exceeds cache capacity %d", S, Smax);
+                  cudaStream_t stream, const int32_t* pos0) {
+    B2_CHECK_ARG(pos0 != nullptr || S <= Smax, "rope_kv_write: S=%d exceeds cache capacity %d", S, Smax);
     B2_CHECK_ARG(D % 16 == 0 && D <= 256, "rope_kv_write: head_dim must be a multiple of 16, <= 256 (got %d)", D);
     B2_CHECK_ARG(((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(kcache) |
                    reinterpret_cast<uintptr_t>(vcache)) & 15) == 0, "rope_kv_write: buffers must be 16-byte aligned");
     B2_CUDA_CHECK(launch_pdl(rope_kv_write_kernel, dim3(B * S), dim3(256), 0, stream, reinterpret_cast<__nv_bfloat16*>(qkv),
-                             reinterpret_cast<__nv_bfloat16*>(kcache), reinterpret_cast<__nv_bfloat16*>(vcache), S, H, D, Smax, theta));
+                             reinterpret_cast<__nv_bfloat16*>(kcache), reinterpret_cast<__nv_bfloat16*>(vcache), pos0, S, H, D, Smax, theta));
     B2_LAUNCH_CHECK();
     return 0;
 }
@@ -919,16 +960,34 @@ int decode_attn_e4m3(const DecodeAttnArgs& a, cudaStream_t stream) {
 }
 
 int kv_quantize_e4m3(const void* ksrc, const void* vsrc, void* k8, void* v8, float* kscale, float* vscale,
-                     const int32_t* seq_lens, int B, int S, int H, int D, int Smax, cudaStream_t stream) {
+                     const int32_t* seq_lens, int B, int S, int H, int D, int Smax, cudaStream_t stream, const int32_t* pos0,
+                     int S_src) {
+    if (S_src == 0) S_src = S;
     B2_CHECK_ARG(D == DA_D, "kv_quantize_e4m3: head_dim must be 128 (got %d)", D);
-    B2_CHECK_ARG(B > 0 && H > 0 && S > 0 && S <= Smax, "kv_quantize_e4m3: B=%d H=%d S=%d Smax=%d", B, H, S, Smax);
+    B2_CHECK_ARG(B > 0 && H > 0 && S > 0 && (pos0 != nullptr || (S <= Smax && S_src == S)),
+                 "kv_quantize_e4m3: B=%d H=%d S=%d S_src=%d Smax=%d", B, H, S, S_src, Smax);
     B2_CHECK_ARG(((reinterpret_cast<uintptr_t>(ksrc) | reinterpret_cast<uintptr_t>(vsrc)) & 15) == 0 &&
                  ((reinterpret_cast<uintptr_t>(k8) | reinterpret_cast<uintptr_t>(v8)) & 7) == 0,
                  "kv_quantize_e4m3: slabs must be 16-byte and caches 8-byte aligned");
     dim3 grid((S + KQ_TILE - 1) / KQ_TILE, H, B);
     B2_CUDA_CHECK(launch_pdl(kv_quantize_e4m3_kernel, grid, dim3(256), 0, stream, reinterpret_cast<const __nv_bfloat16*>(ksrc),
                              reinterpret_cast<const __nv_bfloat16*>(vsrc), reinterpret_cast<uint8_t*>(k8),
-                             reinterpret_cast<uint8_t*>(v8), kscale, vscale, seq_lens, S, H, Smax));
+                             reinterpret_cast<uint8_t*>(v8), kscale, vscale, seq_lens, pos0, S, S_src, H, Smax));
+    B2_LAUNCH_CHECK();
+    return 0;
+}
+
+int kv_dequantize_e4m3(const void* k8, const void* v8, const float* kscale, const float* vscale, const int32_t* pos0, void* kdst,
+                       void* vdst, int B, int H, int Smax, int S_dst, cudaStream_t stream) {
+    B2_CHECK_ARG(k8 && v8 && kscale && vscale && pos0 && kdst && vdst, "kv_dequantize_e4m3: null argument");
+    B2_CHECK_ARG(B > 0 && H > 0 && Smax > 0 && S_dst > 0, "kv_dequantize_e4m3: B=%d H=%d Smax=%d S_dst=%d", B, H, Smax, S_dst);
+    B2_CHECK_ARG(((reinterpret_cast<uintptr_t>(k8) | reinterpret_cast<uintptr_t>(v8)) & 7) == 0 &&
+                 ((reinterpret_cast<uintptr_t>(kdst) | reinterpret_cast<uintptr_t>(vdst)) & 15) == 0,
+                 "kv_dequantize_e4m3: caches must be 8-byte and slabs 16-byte aligned");
+    dim3 grid((S_dst + KQ_TILE - 1) / KQ_TILE, H, B);
+    B2_CUDA_CHECK(launch_pdl(kv_dequantize_e4m3_kernel, grid, dim3(256), 0, stream, reinterpret_cast<const uint8_t*>(k8),
+                             reinterpret_cast<const uint8_t*>(v8), kscale, vscale, pos0, reinterpret_cast<__nv_bfloat16*>(kdst),
+                             reinterpret_cast<__nv_bfloat16*>(vdst), H, Smax, S_dst));
     B2_LAUNCH_CHECK();
     return 0;
 }

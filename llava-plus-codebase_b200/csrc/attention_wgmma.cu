@@ -46,6 +46,7 @@ __device__ __forceinline__ float ex2_approx(float x) {
 
 struct FlashTcParams {
     const int32_t* seq_lens;
+    const int32_t* pos0;  // OFFSET only: absolute position of query row 0 of each sample (keys 0 .. pos0 + t are attended)
     __nv_bfloat16* o;
     int64_t o_bs, o_ts, o_hs;
     int S;
@@ -57,7 +58,10 @@ struct TcCfg {
     static constexpr int SMEM = 5 * TC_BN * D * 2 + 1024 /*align*/ + 128 /*barriers*/;  // Q + 2 K stages + 2 V stages
 };
 
-template <int D, bool CAUSAL>
+// OFFSET: the queries of sample b are a chunk appended at cache position pos0[b] (query row t sits at absolute position
+// pos0[b] + t) and K / V are the whole cache [B][H][Smax][D]. Key tiles stay aligned to absolute position 0; masks compare
+// absolute positions. OFFSET == false is the position-0 kernel (qpos0 folds to 0).
+template <int D, bool CAUSAL, bool OFFSET>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 flash_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                    const __grid_constant__ CUtensorMap tm_v, FlashTcParams p) {
@@ -83,7 +87,9 @@ flash_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
     pdl_trigger();
     pdl_wait();  // q/k/v (and seq_lens) are outputs of upstream kernels (programmatic dependent launch)
     const int len = p.seq_lens != nullptr ? p.seq_lens[b] : p.S;
-    const int kv_end = CAUSAL ? min(len, q0 + TC_BM) : len;
+    const int qpos0 = OFFSET ? p.pos0[b] : 0;
+    const int kv_len = qpos0 + len;  // keys of this sample: [0, kv_len)
+    const int kv_end = CAUSAL ? min(kv_len, qpos0 + q0 + TC_BM) : kv_len;
     const int n_tiles = (kv_end + TC_BN - 1) / TC_BN;  // >= 1 (len >= 1)
 
     if (threadIdx.x == 0) {
@@ -149,14 +155,14 @@ flash_wgmma_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_consta
             wgmma_wait<0>();
             if (lane == 0) mbar_arrive(&k_empty[s]);  // K_j consumed
             // interior tiles need no per-key mask (CTA-uniform test: every key valid for every query row of this CTA)
-            const bool full_tile = (key0 + TC_BN <= len) && (!CAUSAL || key0 + TC_BN - 1 <= q0);
+            const bool full_tile = (key0 + TC_BN <= kv_len) && (!CAUSAL || key0 + TC_BN - 1 <= qpos0 + q0);
             float mx[2] = {-INFINITY, -INFINITY};
             if (!full_tile) {
 #pragma unroll
                 for (int i = 0; i < TC_BN / 2; ++i) {
                     const int key = key0 + frag_col(tid, i);
-                    bool ok = key < len;
-                    if (CAUSAL) ok = ok && (key <= q0 + rows[(i >> 1) & 1]);
+                    bool ok = key < kv_len;
+                    if (CAUSAL) ok = ok && (key <= qpos0 + q0 + rows[(i >> 1) & 1]);
                     if (!ok) sc[i] = -INFINITY;
                 }
             }
@@ -254,21 +260,23 @@ int make_tmap_4d(CUtensorMap* map, const void* ptr, int D, int S, int H, int B, 
     return 0;
 }
 
-template <int D, bool CAUSAL>
+template <int D, bool CAUSAL, bool OFFSET>
 int launch_tc(const FlashArgs& a, cudaStream_t stream) {
+    const int skv = OFFSET ? a.Skv : a.S;  // rows of the K / V views
     CUtensorMap tq, tk, tv;
     B2_TRY(make_tmap_4d(&tq, a.q, D, a.S, a.H, a.B, a.q_ts, a.q_hs, a.q_bs));
-    B2_TRY(make_tmap_4d(&tk, a.k, D, a.S, a.H, a.B, a.k_ts, a.k_hs, a.k_bs));
-    B2_TRY(make_tmap_4d(&tv, a.v, D, a.S, a.H, a.B, a.v_ts, a.v_hs, a.v_bs));
+    B2_TRY(make_tmap_4d(&tk, a.k, D, skv, a.H, a.B, a.k_ts, a.k_hs, a.k_bs));
+    B2_TRY(make_tmap_4d(&tv, a.v, D, skv, a.H, a.B, a.v_ts, a.v_hs, a.v_bs));
     FlashTcParams p;
     p.seq_lens = a.seq_lens;
+    p.pos0 = a.pos0;
     p.o = reinterpret_cast<__nv_bfloat16*>(a.o);
     p.o_bs = a.o_bs; p.o_ts = a.o_ts; p.o_hs = a.o_hs;
     p.S = a.S;
     p.scale_log2 = a.scale * 1.4426950408889634f;
     constexpr int smem = TcCfg<D>::SMEM;
     static bool attr_set = false;
-    auto kern = flash_wgmma_kernel<D, CAUSAL>;
+    auto kern = flash_wgmma_kernel<D, CAUSAL, OFFSET>;
     if (!attr_set) {
         B2_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         attr_set = true;
@@ -285,8 +293,14 @@ int flash_attn_tc_bf16(const FlashArgs& a, cudaStream_t stream) {
     B2_CHECK_ARG(a.D == 64 || a.D == 128, "flash_attn(tc): head_dim must be 64 or 128 (got %d)", a.D);
     B2_CHECK_ARG((a.o_ts % 8) == 0 && (a.o_hs % 8) == 0 && (a.o_bs % 8) == 0 && (reinterpret_cast<uintptr_t>(a.o) & 15) == 0,
                  "flash_attn(tc): output must be 16B aligned with 16B-multiple strides");
-    if (a.D == 64) return a.causal ? launch_tc<64, true>(a, stream) : launch_tc<64, false>(a, stream);
-    return a.causal ? launch_tc<128, true>(a, stream) : launch_tc<128, false>(a, stream);
+    if (a.pos0 != nullptr) {
+        // chunk against a cache: causal, head_dim 128 (the decoder's attention) only
+        B2_CHECK_ARG(a.D == 128 && a.causal && a.Skv >= 1, "flash_attn(tc): offset queries need D=128, causal, Skv >= 1 (D=%d causal=%d Skv=%d)",
+                     a.D, a.causal, a.Skv);
+        return launch_tc<128, true, true>(a, stream);
+    }
+    if (a.D == 64) return a.causal ? launch_tc<64, true, false>(a, stream) : launch_tc<64, false, false>(a, stream);
+    return a.causal ? launch_tc<128, true, false>(a, stream) : launch_tc<128, false, false>(a, stream);
 }
 
 }  // namespace b2

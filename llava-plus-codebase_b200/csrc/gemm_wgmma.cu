@@ -127,6 +127,7 @@ struct EpiParams {
     int ld_out, ld_res, out_fp32;
     // ACT_ROPE_QKV
     const uint32_t* rope_tab;
+    const int32_t* rope_pos0;
     __nv_bfloat16* kcache;
     __nv_bfloat16* vcache;
     int rope_S, rope_H, rope_Smax;
@@ -275,7 +276,16 @@ __device__ __forceinline__ void epilogue_tile(const float (&acc)[GemmCfg<BN>::NC
             for (int hh = 0; hh < 2; ++hh) {
                 const int row = row_lo + 8 * hh;
                 if (row >= M) continue;
-                const int b = row / ep.rope_S, tpos = row - b * ep.rope_S;
+                const int b = row / ep.rope_S;
+                int tpos = row - b * ep.rope_S;
+                if (ep.rope_pos0 != nullptr) {
+                    // chunk at a cache offset: padding rows beyond the cache keep a finite q (last table row), store no k / v
+                    tpos += ep.rope_pos0[b];
+                    if (tpos >= ep.rope_Smax) {
+                        if (part != 0) continue;
+                        tpos = ep.rope_Smax - 1;
+                    }
+                }
                 __nv_bfloat16* dst;
                 if (part == 0) dst = reinterpret_cast<__nv_bfloat16*>(ep.out) + (size_t)row * ep.ld_out + col_base;
                 else dst = (part == 1 ? ep.kcache : ep.vcache) + (((size_t)b * ep.rope_H + head) * ep.rope_Smax + tpos) * 128;
@@ -636,6 +646,7 @@ EpiParams make_epi(const GemmArgs& g) {
     ep.rope_tab = reinterpret_cast<const uint32_t*>(g.rope.table);
     ep.kcache = reinterpret_cast<__nv_bfloat16*>(g.rope.kcache); ep.vcache = reinterpret_cast<__nv_bfloat16*>(g.rope.vcache);
     ep.rope_S = g.rope.S; ep.rope_H = g.rope.H; ep.rope_Smax = g.rope.Smax;
+    ep.rope_pos0 = g.rope.pos0;
     return ep;
 }
 
@@ -684,7 +695,8 @@ int gemm_bf16_2cta(const GemmArgs& g, cudaStream_t stream) {
     B2_TRY(make_tmap_bf16(&tb, g.W, g.N, g.K, g.ldw, BM));  // each CTA of a pair fetches 128 of the tile's 256 W rows
     const EpiParams ep = make_epi(g);
     if (g.act == ACT_ROPE_QKV) {
-        B2_CHECK_ARG(g.rope.table && g.rope.kcache && g.rope.vcache && g.rope.S > 0 && g.rope.H > 0 && g.rope.Smax >= g.rope.S,
+        B2_CHECK_ARG(g.rope.table && g.rope.kcache && g.rope.vcache && g.rope.S > 0 && g.rope.H > 0 &&
+                         (g.rope.pos0 != nullptr || g.rope.Smax >= g.rope.S),
                      "gemm_2cta(rope_qkv): rope arguments missing");
         B2_CHECK_ARG(g.N == 3 * g.rope.H * 128 && (g.rope.H * 128) % 256 == 0 && g.M % g.rope.S == 0 && !g.out_fp32 &&
                          g.bias == nullptr && g.residual == nullptr,

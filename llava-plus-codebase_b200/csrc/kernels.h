@@ -17,6 +17,9 @@ struct RopeQkv {
     void* kcache = nullptr;        // this layer's K slab of the first batch row written
     void* vcache = nullptr;
     int S = 0, H = 0, Smax = 0;
+    // device int32 [B] or null: row t of sample b is position pos0[b] + t (table entry and cache row); rows at or beyond Smax
+    // store no k / v. Smax must not exceed the table's rows.
+    const int32_t* pos0 = nullptr;
 };
 enum { DT_BF16 = 0, DT_F16 = 1, DT_F32 = 2 };
 
@@ -110,6 +113,10 @@ struct FlashArgs {
     const void* v = nullptr; int64_t v_bs = 0, v_ts = 0, v_hs = 0;
     void* o = nullptr;       int64_t o_bs = 0, o_ts = 0, o_hs = 0;
     const int32_t* seq_lens = nullptr;  // device [B] or null (=S)
+    // device [B] or null: query row t of sample b sits at absolute position pos0[b] + t and attends keys 0 .. pos0[b] + t of
+    // k / v, which then hold Skv rows per (b, head) (a KV cache). Causal, D = 128, wgmma kernel only.
+    const int32_t* pos0 = nullptr;
+    int Skv = 0;
     int B = 0, H = 0, S = 0, D = 0;     // S = padded/query length; D in {64, 128}
     int causal = 0;
     float scale = 1.f;
@@ -122,8 +129,10 @@ int flash_attn_mma_bf16(const FlashArgs& a, cudaStream_t stream);  // attention.
 // kcache/vcache: [Bmax, H, Smax, D] for one layer. Positions are 0..S-1 (right-padded rows).
 // (cos, sin) table of rope_kv_write's positions 0..Smax-1 (head_dim D): uint32 [Smax][D/2], bf16 cos | bf16 sin << 16
 int rope_table_build(void* table, int Smax, int D, float theta, cudaStream_t stream);
+// pos0 (device int32 [B] or null): row t of sample b is the token at absolute position pos0[b] + t (its RoPE angle and its
+// cache row); rows at or beyond Smax are rotated but not stored. pos0 == null: positions t, S <= Smax.
 int rope_kv_write(void* qkv, void* kcache, void* vcache, int B, int S, int H, int D, int Smax, float theta,
-                  cudaStream_t stream);
+                  cudaStream_t stream, const int32_t* pos0 = nullptr);
 
 // decode: q/k/v of the new token from qkv [B, 3*H*D]; RoPE at position cur_len[b]; append k,v to the cache;
 // split-KV attention over cur_len[b]+1 keys; out [B, H*D] bf16.
@@ -145,8 +154,15 @@ int decode_attn_e4m3_ctas_per_sm();
 int decode_attn_e4m3(const DecodeAttnArgs& a, cudaStream_t stream);
 // prefill cache write of an e4m3 cache: roped bf16 K / V of one layer, [B, H, S, D] contiguous, -> rows t < seq_lens[b]
 // (device, null = S) of k8 / v8 [B, H, Smax, D] bytes and kscale / vscale [B, H, Smax]
+// With pos0 (device int32 [B]): the slabs are [B, H, S_src, D] (0 = S) and chunk row t < seq_lens[b] is read from and stored
+// at row pos0[b] + t; rows outside the slab or the cache are skipped.
 int kv_quantize_e4m3(const void* ksrc, const void* vsrc, void* k8, void* v8, float* kscale, float* vscale,
-                     const int32_t* seq_lens, int B, int S, int H, int D, int Smax, cudaStream_t stream);
+                     const int32_t* seq_lens, int B, int S, int H, int D, int Smax, cudaStream_t stream,
+                     const int32_t* pos0 = nullptr, int S_src = 0);
+// the stored prefix as bf16: rows t < pos0[b] (device int32 [B]) of k8 / v8 [B, H, Smax, 128] and their scales ->
+// bf16(float(q) * scale) at row t of kdst / vdst [B, H, S_dst, 128]
+int kv_dequantize_e4m3(const void* k8, const void* v8, const float* kscale, const float* vscale, const int32_t* pos0, void* kdst,
+                       void* vdst, int B, int H, int Smax, int S_dst, cudaStream_t stream);
 
 // ---- persistent decode-step megakernel (decode_mega.cu), batch <= 8 ------------------------------------
 struct MegaLayer {

@@ -102,6 +102,7 @@ struct b2_model {
     DevBuf v_col, v_patch, v_hidden, v_xn, v_qkv, v_attn, v_mlp, v_feats, p_mid, p_done;
     // LLaMA workspace
     DevBuf x, xn, qkv, attn, act, last_idx, xlast, logits, splice_idx;
+    DevBuf chunk_pos;  // b2_prefill_at: int32 [2][max_batch] = start position, then chunk length, of each sample
     // encode_images replays a CUDA graph per chunk size (~190 launches per image, 5-20 us each at B = 1: the host cannot
     // keep the GPU fed launch by launch). Inputs/outputs are staged through fixed buffers so the captured pointers stay valid.
     DevBuf enc_pixels, enc_out;
@@ -785,7 +786,7 @@ int b2_init(int device) {
 }
 
 const char* b2_last_error(void) { return g_err; }
-int b2_version(void) { return 2; }
+int b2_version(void) { return 3; }
 unsigned long long b2_launch_count(void) { return g_launch_count; }
 
 int b2_model_create(const b2_model_desc* desc, b2_model** out) {
@@ -940,6 +941,7 @@ int b2_model_finalize(b2_model* m) {
     B2_TRY(m->attn.alloc(rows * h * 2));
     B2_TRY(m->act.alloc(rows * d.inter * 2));
     B2_TRY(m->last_idx.alloc((size_t)d.max_batch * 4));
+    B2_TRY(m->chunk_pos.alloc((size_t)d.max_batch * 2 * 4));
     B2_TRY(m->splice_idx.alloc(rows * 4));
     B2_TRY(m->xlast.alloc((size_t)d.max_batch * h * 2));
     B2_TRY(m->logits.alloc((size_t)d.max_batch * d.vocab * 4));
@@ -960,7 +962,7 @@ int b2_model_destroy(b2_model* m) {
     DevBuf* top[] = {&m->patch_w, &m->cls, &m->pos, &m->pre_g, &m->pre_b, &m->p0_w, &m->p0_b, &m->p2_w, &m->p2_b,
                      &m->embed, &m->final_norm, &m->lm_head, &m->v_col, &m->v_patch, &m->v_hidden, &m->v_xn,
                      &m->v_qkv, &m->v_attn, &m->v_mlp, &m->v_feats, &m->p_mid, &m->p_done, &m->enc_pixels, &m->enc_out, &m->x, &m->xn, &m->qkv, &m->attn,
-                     &m->act, &m->last_idx, &m->xlast, &m->logits, &m->splice_idx, &m->lm_head8, &m->s_head, &m->xq8, &m->xscale,
+                     &m->act, &m->last_idx, &m->chunk_pos, &m->xlast, &m->logits, &m->splice_idx, &m->lm_head8, &m->s_head, &m->xq8, &m->xscale,
                      &m->kstage, &m->vstage};
     for (DevBuf* b : top) b->free();
     for (VitLayer& L : m->vit) {
@@ -1263,11 +1265,16 @@ int b2_async_error(b2_model* m, int* code_out) {
 
 int b2_prefill(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* seq_lens_host, int B, int S,
                void* logits_out, int logits_mode, void* stream) {
-    return b2_prefill_slots(m, kv, embeds, seq_lens_host, B, S, 0, logits_out, logits_mode, stream);
+    return b2_prefill_at(m, kv, embeds, nullptr, seq_lens_host, B, S, 0, logits_out, logits_mode, stream);
 }
 
 int b2_prefill_slots(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* seq_lens_host, int B, int S, int slot0,
                      void* logits_out, int logits_mode, void* stream) {
+    return b2_prefill_at(m, kv, embeds, nullptr, seq_lens_host, B, S, slot0, logits_out, logits_mode, stream);
+}
+
+int b2_prefill_at(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* start_host, const int32_t* seq_lens_host, int B,
+                  int S, int slot0, void* logits_out, int logits_mode, void* stream) {
     B2_CHECK_ARG(m && kv && embeds && kv->m == m, "b2_prefill: bad handle");
     B2_CHECK_ARG(m->finalized, "b2_prefill: model not finalized");
     B2_CHECK_ARG(B >= 1 && slot0 >= 0 && slot0 + B <= kv->max_batch && S >= 1 && S <= kv->max_seq,
@@ -1281,21 +1288,39 @@ int b2_prefill_slots(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* 
     const b2_model_desc& d = m->d;
     const int h = d.hidden, I = d.inter, H = d.heads, V = d.vocab, T = B * S;
 
-    std::vector<int32_t> lens(B), last(B);
+    std::vector<int32_t> lens(B), last(B), start(B, 0), total(B);
+    int max_start = 0;
     for (int b = 0; b < B; ++b) {
         lens[b] = seq_lens_host ? seq_lens_host[b] : S;
         B2_CHECK_ARG(lens[b] >= 1 && lens[b] <= S, "b2_prefill: seq_lens[%d]=%d out of range (S=%d)", b, lens[b], S);
+        if (start_host != nullptr) {
+            start[b] = start_host[b];
+            B2_CHECK_ARG(start[b] >= 0 && start[b] <= kv->len_host[slot0 + b],
+                         "b2_prefill_at: start[%d]=%d outside [0, current length %d]", b, start[b], kv->len_host[slot0 + b]);
+            B2_CHECK_ARG(start[b] + lens[b] <= kv->max_seq, "b2_prefill_at: start[%d]=%d + %d tokens exceed the cache (max_seq=%d)",
+                         b, start[b], lens[b], kv->max_seq);
+        }
+        max_start = start[b] > max_start ? start[b] : max_start;
+        total[b] = start[b] + lens[b];
         last[b] = b * S + lens[b] - 1;
     }
+    // a chunk at position 0 everywhere is an ordinary prefill (the same kernels, bit for bit)
+    const bool offset = max_start > 0;
+    const bool q8 = kv->e4m3();
+    // e4m3 cache: the producers below write one layer of roped bf16 K / V into the staging slab [B][H][kv_pitch][128] (a cache
+    // with Smax = kv_pitch), attention reads it there, and kv_quantize_e4m3 then stores the layer's chunk rows and scales. At an
+    // offset the slab also holds the stored prefix, dequantised (rows [0, start)), in front of the chunk's rows.
+    const int kv_pitch = !q8 ? kv->pitch : (offset ? (max_start + S < kv->max_seq ? max_start + S : kv->max_seq) : S);
+    B2_CHECK_ARG(!q8 || (size_t)B * kv_pitch <= (size_t)d.max_batch * d.max_seq,
+                 "b2_prefill_at: %d samples x %d rows exceed the staging slab (%d rows)", B, kv_pitch, d.max_batch * d.max_seq);
     B2_TRY(ws_enter(m, st));
     // lengths / last-row indices travel as kernel parameters: no pinned staging, no stream sync in this call
-    B2_TRY(set_i32_pairs(kv->len_dev.as<int32_t>() + slot0, lens.data(), m->last_idx.as<int32_t>(), last.data(), B, st));
-    for (int b = 0; b < B; ++b) kv->len_host[slot0 + b] = lens[b];
+    B2_TRY(set_i32_pairs(kv->len_dev.as<int32_t>() + slot0, total.data(), m->last_idx.as<int32_t>(), last.data(), B, st));
+    int32_t* pos_dev = m->chunk_pos.as<int32_t>();  // [0, B): start, [max_batch, +B): chunk length
+    int32_t* clen_dev = pos_dev + d.max_batch;
+    if (offset) B2_TRY(set_i32_pairs(pos_dev, start.data(), clen_dev, lens.data(), B, st));
+    for (int b = 0; b < B; ++b) kv->len_host[slot0 + b] = total[b];
     const size_t slot_rows = (size_t)slot0 * H * kv->pitch;  // cache rows in front of the first slot this call fills
-    const bool q8 = kv->e4m3();
-    // e4m3 cache: the producers below write one layer of roped bf16 K / V into the staging slab [B][H][S][128] (a cache with
-    // Smax = S), attention reads it there, and kv_quantize_e4m3 then stores the layer's cache rows and scales
-    const int kv_pitch = q8 ? S : kv->pitch;
 
     B2_CUDA_CHECK(cudaMemcpyAsync(m->x.p, embeds, (size_t)T * h * 2, cudaMemcpyDeviceToDevice, st));
     // RoPE + KV write fused into the QKV GEMM where the CTA-pair kernel is the one that runs anyway (M >= 512; 256-column pair
@@ -1306,6 +1331,11 @@ int b2_prefill_slots(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* 
         LlamaLayer& L = m->ll[l];
         bf16* kc = q8 ? m->kstage.as<bf16>() : reinterpret_cast<bf16*>(kv->k_layer(l)) + slot_rows * m->hd;
         bf16* vc = q8 ? m->vstage.as<bf16>() : reinterpret_cast<bf16*>(kv->v_layer(l)) + slot_rows * m->hd;
+        const size_t row0 = (size_t)l * kv->layer_rows() + slot_rows;  // e4m3: first scale / row of this layer's slots
+        if (q8 && offset)
+            B2_TRY(kv_dequantize_e4m3(kv->k.as<uint8_t>() + row0 * m->hd, kv->v.as<uint8_t>() + row0 * m->hd,
+                                      kv->kscale.as<float>() + row0, kv->vscale.as<float>() + row0, pos_dev, kc, vc, B, H,
+                                      kv->pitch, kv_pitch, st));
         B2_TRY(rmsnorm_bf16(m->x.p, h, L.ln1.p, m->xn.p, T, h, d.rms_eps, st));
         if (rope_fused) {
             // QKV projection with RoPE and the cache write in its epilogue (CTA-pair kernel): q -> qkv buffer, k / v -> cache
@@ -1313,25 +1343,27 @@ int b2_prefill_slots(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* 
             g.A = m->xn.p; g.lda = h; g.W = L.wqkv.p; g.ldw = h; g.out = m->qkv.p; g.ld_out = 3 * h;
             g.M = T; g.N = 3 * h; g.K = h; g.act = ACT_ROPE_QKV;
             g.rope.table = kv->rope_tab.p; g.rope.kcache = kc; g.rope.vcache = vc; g.rope.S = S; g.rope.H = H; g.rope.Smax = kv_pitch;
+            g.rope.pos0 = offset ? pos_dev : nullptr;
             B2_TRY(gemm_bf16_2cta(g, st));
         } else {
             B2_TRY(gemm(m->xn.p, h, L.wqkv.p, h, nullptr, nullptr, 0, m->qkv.p, 3 * h, 0, T, 3 * h, h, ACT_NONE, st));
-            B2_TRY(rope_kv_write(m->qkv.p, kc, vc, B, S, H, m->hd, kv_pitch, d.rope_theta, st));
+            B2_TRY(rope_kv_write(m->qkv.p, kc, vc, B, S, H, m->hd, kv_pitch, d.rope_theta, st, offset ? pos_dev : nullptr));
         }
         FlashArgs fa;
         fa.q = m->qkv.p; fa.q_bs = (int64_t)S * 3 * h; fa.q_ts = 3 * h; fa.q_hs = m->hd;
         fa.k = kc; fa.k_bs = (int64_t)H * kv_pitch * m->hd; fa.k_ts = m->hd; fa.k_hs = (int64_t)kv_pitch * m->hd;
         fa.v = vc; fa.v_bs = fa.k_bs; fa.v_ts = m->hd; fa.v_hs = fa.k_hs;
         fa.o = m->attn.p; fa.o_bs = (int64_t)S * h; fa.o_ts = h; fa.o_hs = m->hd;
-        fa.seq_lens = kv->len_dev.as<int32_t>() + slot0;
+        fa.seq_lens = offset ? clen_dev : kv->len_dev.as<int32_t>() + slot0;
+        if (offset) { fa.pos0 = pos_dev; fa.Skv = kv_pitch; }
         fa.B = B; fa.H = H; fa.S = S; fa.D = m->hd; fa.causal = 1;
         fa.scale = 1.0f / sqrtf((float)m->hd);
         B2_TRY(flash_attn_bf16(fa, st));
         if (q8) {
-            const size_t row0 = (size_t)l * kv->layer_rows() + slot_rows;
             B2_TRY(kv_quantize_e4m3(kc, vc, kv->k.as<uint8_t>() + row0 * m->hd, kv->v.as<uint8_t>() + row0 * m->hd,
                                     kv->kscale.as<float>() + row0, kv->vscale.as<float>() + row0,
-                                    kv->len_dev.as<int32_t>() + slot0, B, S, H, m->hd, kv->pitch, st));
+                                    offset ? clen_dev : kv->len_dev.as<int32_t>() + slot0, B, S, H, m->hd, kv->pitch, st,
+                                    offset ? pos_dev : nullptr, kv_pitch));
         }
         B2_TRY(gemm(m->attn.p, h, L.wo.p, h, nullptr, m->x.p, h, m->x.p, h, 0, T, h, h, ACT_NONE, st));
         B2_TRY(rmsnorm_bf16(m->x.p, h, L.ln2.p, m->xn.p, T, h, d.rms_eps, st));
@@ -1739,6 +1771,40 @@ int b2_op_kv_quantize_e4m3(const void* kstage, const void* vstage, void* k8, voi
                            const int32_t* seq_lens, int B, int S, int H, int Smax, void* stream) {
     B2_CHECK_ARG(kstage && vstage && k8 && v8 && kscale && vscale, "b2_op_kv_quantize_e4m3: null argument");
     return kv_quantize_e4m3(kstage, vstage, k8, v8, kscale, vscale, seq_lens, B, S, H, 128, Smax, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2_op_flash_attn_kv(const void* q, const void* kcache, const void* vcache, void* o, const int32_t* pos0, const int32_t* seq_lens,
+                        int B, int S, int H, int Smax, float scale, void* stream) {
+    B2_CHECK_ARG(q && kcache && vcache && o && pos0, "b2_op_flash_attn_kv: null argument");
+    B2_CHECK_ARG(B >= 1 && S >= 1 && H >= 1 && Smax >= 1, "b2_op_flash_attn_kv: bad shape B=%d S=%d H=%d Smax=%d", B, S, H, Smax);
+    const int D = 128;
+    FlashArgs fa;
+    fa.q = q; fa.q_bs = (int64_t)S * H * D; fa.q_ts = (int64_t)H * D; fa.q_hs = D;
+    fa.k = kcache; fa.k_bs = (int64_t)H * Smax * D; fa.k_ts = D; fa.k_hs = (int64_t)Smax * D;
+    fa.v = vcache; fa.v_bs = fa.k_bs; fa.v_ts = D; fa.v_hs = fa.k_hs;
+    fa.o = o; fa.o_bs = fa.q_bs; fa.o_ts = fa.q_ts; fa.o_hs = D;
+    fa.seq_lens = seq_lens; fa.pos0 = pos0; fa.Skv = Smax;
+    fa.B = B; fa.H = H; fa.S = S; fa.D = D; fa.causal = 1; fa.scale = scale;
+    return flash_attn_bf16(fa, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2_op_rope_kv_write_at(void* qkv, void* kcache, void* vcache, const int32_t* pos0, int B, int S, int H, int D, int Smax,
+                           float theta, void* stream) {
+    B2_CHECK_ARG(qkv && kcache && vcache && pos0, "b2_op_rope_kv_write_at: null argument");
+    return rope_kv_write(qkv, kcache, vcache, B, S, H, D, Smax, theta, reinterpret_cast<cudaStream_t>(stream), pos0);
+}
+
+int b2_op_kv_dequantize_e4m3(const void* k8, const void* v8, const float* kscale, const float* vscale, const int32_t* pos0,
+                             void* kdst, void* vdst, int B, int H, int Smax, int S_dst, void* stream) {
+    return kv_dequantize_e4m3(k8, v8, kscale, vscale, pos0, kdst, vdst, B, H, Smax, S_dst, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2_op_kv_quantize_e4m3_at(const void* kstage, const void* vstage, void* k8, void* v8, float* kscale, float* vscale,
+                              const int32_t* pos0, const int32_t* seq_lens, int B, int S, int S_src, int H, int Smax, void* stream) {
+    B2_CHECK_ARG(kstage && vstage && k8 && v8 && kscale && vscale && pos0, "b2_op_kv_quantize_e4m3_at: null argument");
+    B2_CHECK_ARG(S_src >= 1, "b2_op_kv_quantize_e4m3_at: S_src=%d", S_src);
+    return kv_quantize_e4m3(kstage, vstage, k8, v8, kscale, vscale, seq_lens, B, S, H, 128, Smax, reinterpret_cast<cudaStream_t>(stream),
+                            pos0, S_src);
 }
 
 int b2_op_interleave_gate_up(const void* gate, const void* up, void* out, int I, int h, void* stream) {

@@ -91,6 +91,7 @@ SIGNATURES = {
     "b2_op_sample": (_i32, [_vp, _i32, _i32, _c.POINTER(Sampling), _i32, _vp, _vp]),
     "b2_prefill": (_i32, [_vp, _vp, _vp, _c.POINTER(_c.c_int32), _i32, _i32, _vp, _i32, _vp]),
     "b2_prefill_slots": (_i32, [_vp, _vp, _vp, _c.POINTER(_c.c_int32), _i32, _i32, _i32, _vp, _i32, _vp]),
+    "b2_prefill_at": (_i32, [_vp, _vp, _vp, _c.POINTER(_c.c_int32), _c.POINTER(_c.c_int32), _i32, _i32, _i32, _vp, _i32, _vp]),
     "b2_batch_begin": (_i32, [_vp, _vp, _i32, _vp]),
     "b2_batch_set_row": (_i32, [_vp, _vp, _i32, _i32, _c.POINTER(Sampling), _i32, _vp]),
     "b2_decode_step": (_i32, [_vp, _vp, _vp, _i32, _vp, _vp, _vp]),
@@ -108,11 +109,15 @@ SIGNATURES = {
     "b2_op_rmsnorm": (_i32, [_vp, _vp, _vp, _i32, _i32, _f32, _vp]),
     "b2_op_flash_attn": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp]),
     "b2_op_rope_kv_write": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp]),
+    "b2_op_flash_attn_kv": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _vp]),
+    "b2_op_rope_kv_write_at": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp]),
     "b2_op_decode_attn": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _f32, _vp]),
     "b2_op_decode_attn_scratch_bytes": (_i64, [_i32, _i32, _i32]),
     "b2_op_decode_attn_e4m3": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _f32, _vp]),
     "b2_op_decode_attn_nsplit": (_i32, [_i32, _i32, _i32, _i32]),
     "b2_op_kv_quantize_e4m3": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
+    "b2_op_kv_quantize_e4m3_at": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "b2_op_kv_dequantize_e4m3": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
     "b2_op_interleave_gate_up": (_i32, [_vp, _vp, _vp, _i32, _i32, _vp]),
     "b2_op_im2col": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _vp]),
 }
@@ -346,21 +351,27 @@ class Engine:
         if self.take_async_error():
             raise ValueError(last_error())
 
-    def prefill(self, kv, embeds, seq_lens=None, logits_mode=LOGITS_LAST, slot0=0):
-        """`slot0`: first cache slot to fill (continuous batching); the other slots keep their contents."""
+    def prefill(self, kv, embeds, seq_lens=None, logits_mode=LOGITS_LAST, slot0=0, start=None):
+        """`slot0`: first cache slot to fill (continuous batching); the other slots keep their contents. `start` (list of B
+        ints, or None = all 0): cache position where each sample's chunk goes (b2_prefill_at); the cache rows in front of it
+        are attended, a start below the slot's current length rewinds it."""
         embeds = self._bf16(embeds)
         B, S = embeds.shape[0], embeds.shape[1]
-        lens = None
+        lens = pos = None
         if seq_lens is not None:
             lens = (_c.c_int32 * B)(*[int(x) for x in seq_lens])
+        if start is not None:
+            if len(start) != B:
+                raise ValueError(f"start has {len(start)} entries for a batch of {B}")
+            pos = (_c.c_int32 * B)(*[int(x) for x in start])
         logits = None
         if logits_mode == LOGITS_LAST:
             logits = torch.empty(B, self.vocab, dtype=torch.float32, device=self.device)
         elif logits_mode == LOGITS_ALL:
             logits = torch.empty(B, S, self.vocab, dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.index):
-            check(self.lib.b2_prefill_slots(self.handle, kv.handle, ptr(embeds), lens, B, S, int(slot0), ptr(logits), logits_mode,
-                                            stream_ptr()), "b2_prefill")
+            check(self.lib.b2_prefill_at(self.handle, kv.handle, ptr(embeds), pos, lens, B, S, int(slot0), ptr(logits), logits_mode,
+                                         stream_ptr()), "b2_prefill")
         return logits
 
     def decode_step(self, kv, tokens, want_logits=True):

@@ -17,6 +17,7 @@ import threading
 import weakref
 from typing import List, Optional, Tuple, Union
 
+import numpy as np
 import torch
 import torch.nn as nn
 from transformers import AutoConfig, LlamaConfig
@@ -24,7 +25,10 @@ from transformers.modeling_outputs import CausalLMOutputWithPast
 
 from ..llava_arch import LlavaMetaModel, LlavaMetaForCausalLM
 from ..multimodal_encoder.clip_encoder import _Holder, _read_checkpoint_dir
-from ..._b2 import Engine, KVCache, LOGITS_ALL, LOGITS_LAST, ERR_SPLICE_SLOTS, kv_dtype_code, last_error, make_sampling
+from ..._b2 import Engine, KVCache, LOGITS_ALL, LOGITS_LAST, ERR_SPLICE_SLOTS, INT32_MIN, kv_dtype_code, last_error, make_sampling
+from ..._b2 import prefix as _prefix
+from ...constants import IMAGE_TOKEN_INDEX
+from ..llava_arch import build_source_index
 
 
 class LlavaConfig(LlamaConfig):
@@ -41,6 +45,11 @@ class _KVPool:
         self.engine, self.max_batch, self.max_seq, self.cap, self.dtype = engine, max_batch, max_seq, max(1, int(cap)), dtype
         self._cond = threading.Condition()
         self._free, self._made = [], 0
+        self._records = {}   # id(free cache) -> (record of its rows, event recorded at release); prefix reuse only
+        # conversation prefix reuse (generate() with config.b2_prefix_cache): spliced rows taken over from a released cache,
+        # and images whose encode_images was skipped because they lay inside those rows
+        self.reused_positions = 0
+        self.skipped_encodes = 0
 
     def acquire(self):
         with self._cond:
@@ -57,8 +66,49 @@ class _KVPool:
                 self._cond.notify()
             raise
 
-    def release(self, kv):
+    def acquire_prefix(self, items, rows_per_image):
+        """acquire() for a prompt whose spliced items are `items` (llava/_b2/prefix.py): the free cache holding the longest
+        reusable prefix of it, else a new cache while fewer than `cap` exist, else the least recently released one.
+        Returns (kv, rows to reuse, event recorded when the cache was released)."""
         with self._cond:
+            while True:
+                if self._free:
+                    recs = [self._records.get(id(kv), (None, None))[0] for kv in self._free]
+                    i, m = _prefix.select(recs, items, rows_per_image)
+                    if m > 0 or self._made >= self.cap:
+                        kv = self._free.pop(i)
+                        ev = self._records.pop(id(kv), (None, None))[1]
+                        return kv, m, (ev if m > 0 else None)
+                if self._made < self.cap:
+                    self._made += 1
+                    break
+                self._cond.wait()
+        try:
+            kv = _new_kv(self.engine, self.max_batch, self.max_seq, self.dtype)
+        except Exception:
+            with self._cond:
+                self._made -= 1
+                self._cond.notify()
+            raise
+        return kv, 0, None
+
+    def count_reuse(self, rows, images):
+        with self._cond:
+            self.reused_positions += int(rows)
+            self.skipped_encodes += int(images)
+
+    def release(self, kv, record=None):
+        """`record`: what the cache's rows hold (prefix.record_after_generation), or None. An event on the releasing stream
+        orders the next user's prefill after the decode steps this call still has queued (they write rows past the record)."""
+        ev = None
+        if record is not None:
+            ev = torch.cuda.Event()
+            ev.record(torch.cuda.current_stream(self.engine.device))
+        with self._cond:
+            if record is not None:
+                self._records[id(kv)] = (record, ev)
+            else:
+                self._records.pop(id(kv), None)
             self._free.append(kv)
             self._cond.notify()
 
@@ -329,18 +379,14 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
 
         # ---- decode step: [B,1] ids against an engine cache ----
         if inputs_embeds is None and past_key_values is not None and input_ids is not None and input_ids.shape[1] == 1:
-            if isinstance(past_key_values, PastKeyValues):
-                if not past_key_values.valid:
-                    raise RuntimeError("this past_key_values was recycled by a later forward(use_cache=True): the model keeps "
-                                       "config.b2_forward_caches (default 2) forward caches alive at a time")
-                kv = past_key_values.kv
-            elif isinstance(past_key_values, KVCache):
-                kv = past_key_values
-            else:
-                raise ValueError("past_key_values must be the cache object returned by a previous forward of this model")
+            kv = self._resolve_cache(past_key_values)
             logits = engine.decode_step(kv, input_ids.reshape(-1))
             logits = logits.unsqueeze(1)
             return self._output(logits, past_key_values, labels, return_dict)
+
+        if past_key_values is not None:
+            return self._forward_continue(engine, input_ids, inputs_embeds, attention_mask, past_key_values, images, labels,
+                                          return_dict)
 
         if inputs_embeds is None:
             (input_ids, position_ids, attention_mask, past_key_values, inputs_embeds, labels) = \
@@ -348,8 +394,6 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             if inputs_embeds is None:  # text-only (no images / no tower): plain embedding lookup on the engine
                 ids = input_ids.to(torch.int32).reshape(-1).to(engine.device)
                 inputs_embeds = engine.splice(ids, None, input_ids.shape[0], input_ids.shape[1])
-        if past_key_values is not None:
-            raise NotImplementedError("chunked prefill against an existing cache is not part of the reference's call pattern")
 
         B, S = inputs_embeds.shape[0], inputs_embeds.shape[1]
         lens, left = None, False
@@ -365,6 +409,37 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         if left:
             logits = torch.stack([torch.roll(logits[b], shifts=(S - lens[b]), dims=0) for b in range(B)])
         return self._output(logits, lease if use_cache is not False else None, labels, return_dict)
+
+    def _forward_continue(self, engine, input_ids, inputs_embeds, attention_mask, past_key_values, images, labels, return_dict):
+        """HF continuation: the [B, n] chunk is appended to each row's own cache length (b2_prefill_at); image placeholders
+        in the chunk are spliced like a prompt's. Returns logits [B, n', V] (n' = spliced chunk length) and the same cache."""
+        kv = self._resolve_cache(past_key_values)
+        if attention_mask is not None and not bool(attention_mask.bool().all()):
+            raise NotImplementedError("a padded attention_mask on a chunk appended to a cache is not supported")
+        lens = None
+        if inputs_embeds is None:
+            embeds, lens = self._prepare_multimodal(input_ids, None, None, None, None, images)
+            inputs_embeds = embeds[4]
+            if inputs_embeds is None:  # text-only chunk: plain embedding lookup on the engine
+                ids = input_ids.to(torch.int32).reshape(-1).to(engine.device)
+                inputs_embeds = engine.splice(ids, None, input_ids.shape[0], input_ids.shape[1])
+                lens = None
+        B, S = inputs_embeds.shape[0], inputs_embeds.shape[1]
+        start = kv.lengths(B)
+        self._check_limits(engine, B, max(start[b] + (S if lens is None else lens[b]) for b in range(B)))
+        logits = engine.prefill(kv, inputs_embeds, lens, LOGITS_ALL, start=start)
+        return self._output(logits, past_key_values, labels, return_dict)
+
+    @staticmethod
+    def _resolve_cache(past_key_values):
+        if isinstance(past_key_values, PastKeyValues):
+            if not past_key_values.valid:
+                raise RuntimeError("this past_key_values was recycled by a later forward(use_cache=True): the model keeps "
+                                   "config.b2_forward_caches (default 2) forward caches alive at a time")
+            return past_key_values.kv
+        if isinstance(past_key_values, KVCache):
+            return past_key_values
+        raise ValueError("past_key_values must be the cache object returned by a previous forward of this model")
 
     def _output(self, logits, kv, labels, return_dict):
         loss = None
@@ -485,7 +560,16 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 streamer.end()
             return torch.cat([prompt, new_tokens.to(device=prompt.device, dtype=prompt.dtype)], dim=1)
 
-        kv = self._pool.acquire()  # exclusive for this call (concurrent generate() threads each get their own)
+        # conversation prefix reuse (opt-in, batch 1): the part of the prompt a released cache already holds is not prefilled again
+        plan = None
+        if B == 1 and self._prefix_cache_on() and (attention_mask is None or bool(attention_mask.bool().all())):
+            plan = self._prefix_plan(prompt, images)
+        reuse, released_ev = 0, None
+        if plan is not None:
+            kv, reuse, released_ev = self._pool.acquire_prefix(plan["items"], engine.num_patches)
+        else:
+            kv = self._pool.acquire()  # exclusive for this call (concurrent generate() threads each get their own)
+        record = None
         try:
             # ---- prefill: splice + decoder, last-position logits only; token 0 is chosen on the device ----
             def prefill(force_host):
@@ -511,7 +595,11 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 if prof: prof.mark("prefill + first token")
                 return speculative
 
-            speculative = prefill(False)
+            if plan is not None:
+                self._prefill_reusing(engine, kv, plan, reuse, released_ev, sampling, max_new_tokens)
+                speculative = False
+            else:
+                speculative = prefill(False)
             err = engine.take_async_error()
             if speculative and (err & ERR_SPLICE_SLOTS):
                 # the rows do not hold n_images / B placeholders each: the shape-only output length was wrong. Redo on the
@@ -529,13 +617,87 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                                         run_ahead=int(getattr(self.config, "b2_run_ahead", 8)), begun=True)
             engine.check_async_error()
             if prof: prof.mark("decode")
+            if plan is not None:
+                items = [it if isinstance(it, int) else it.detach().clone() for it in plan["items"]]
+                record = _prefix.record_after_generation(items, new_tokens[0].tolist())
         finally:
-            self._pool.release(kv)
+            self._pool.release(kv, record)
         if streamer is not None:
             streamer.end()
         out = torch.cat([prompt, new_tokens.to(device=prompt.device, dtype=prompt.dtype)], dim=1)
         if prof: prof.mark("ids to caller"); prof.report()
         return out
+
+    def _prefix_cache_on(self):
+        """config.b2_prefix_cache or B2_PREFIX_CACHE=1 (off by default: logits of reused answer rows, which the decode kernels
+        wrote, differ from a fresh prefill's by bf16 rounding). Not used when config.b2_continuous_batching routes generate()
+        to the batcher."""
+        v = getattr(self.config, "b2_prefix_cache", None)
+        return bool(v) if v is not None else os.environ.get("B2_PREFIX_CACHE") == "1"
+
+    def _prefix_plan(self, prompt, images):
+        """The spliced items of a batch-1 prompt (llava/_b2/prefix.py), or None when the prompt is outside what the host splice
+        reproduces exactly here (placeholders and image slots do not pair up, truncation, negative ids without images)."""
+        ids = [int(t) for t in prompt[0].tolist()]
+        tower = self.get_vision_tower()
+        if images is None or tower is None:
+            return None if any(t < 0 for t in ids) else {"items": ids, "slots": [], "images": None}
+        if isinstance(images, (list, tuple)):
+            slots = list(images)
+            if any(not torch.is_tensor(x) or x.dim() != 4 for x in slots):
+                return None
+        elif images.dim() in (4, 5):
+            slots = [images[j] for j in range(images.shape[0])]
+        else:
+            return None
+        if sum(t == IMAGE_TOKEN_INDEX for t in ids) != len(slots) or len(ids) < 2:
+            return None
+        it = iter(slots)
+        items = [next(it) if t == IMAGE_TOKEN_INDEX else t for t in ids]
+        total = sum(_prefix.item_rows(x, tower.num_patches) for x in items)
+        max_len = getattr(self.config, "tokenizer_model_max_length", None)
+        if max_len is not None and total > max_len:
+            return None
+        return {"items": items, "slots": slots, "images": images}
+
+    def _prefill_reusing(self, engine, kv, plan, m, released_ev, sampling, max_new_tokens):
+        """Prefill of a planned prompt that keeps the first m spliced rows of `kv`: image slots wholly inside them are not
+        encoded, rows [m, L) are spliced on the host-index path and prefilled at position m (b2_prefill_at). m == 0 is an
+        ordinary prefill from position 0. Chooses and publishes token 0 like generate()'s own prefill."""
+        P = engine.num_patches
+        items, slots = plan["items"], plan["slots"]
+        rows = [_prefix.item_rows(x, P) for x in slots]
+        L = sum(_prefix.item_rows(x, P) for x in items)
+        self._check_limits(engine, 1, L + max_new_tokens)
+        ends, pos = [], 0
+        for x in items:
+            pos += _prefix.item_rows(x, P)
+            if not isinstance(x, int):
+                ends.append(pos)
+        skip = sum(e <= m for e in ends)       # leading slots that lie wholly inside the reused rows
+        if slots:
+            ids_np = np.asarray([[IMAGE_TOKEN_INDEX if not isinstance(x, int) else x for x in items]], dtype=np.int64)
+            src = build_source_index(ids_np, np.ones_like(ids_np, dtype=bool), np.zeros_like(ids_np), sum(rows), rows, None,
+                                     "right", vocab_size=self.get_model().embed_tokens.weight.shape[0])[0][0]
+            chunk = _prefix.chunk_source_index(src, m, sum(rows[:skip]), INT32_MIN)
+        else:  # text only: the ids are the embedding rows (out-of-range ids are flagged by the splice kernel)
+            chunk = np.asarray(items[m:], dtype=np.int32)
+        feats = None
+        if skip < len(slots):
+            images = plan["images"]
+            todo = images[skip:] if torch.is_tensor(images) and images.dim() == 4 else list(slots[skip:])
+            feats, _ = self._image_features(todo)
+        embeds = engine.splice(torch.from_numpy(chunk).to(engine.device), feats, 1, L - m)
+        if m > 0:
+            if released_ev is not None:
+                torch.cuda.current_stream(engine.device).wait_event(released_ev)
+            logits = engine.prefill(kv, embeds, None, LOGITS_LAST, start=[m])
+            self._pool.count_reuse(m, sum(x.shape[0] if x.dim() == 4 else 1 for x in slots[:skip]))
+        else:
+            kv.reset()
+            logits = engine.prefill(kv, embeds, None, LOGITS_LAST)
+        engine.stream_begin(kv, logits, sampling)
+        engine.stream_wait(kv, 0, 1)
 
     # ------------------------------------------------------------------ checkpoints
     @classmethod
