@@ -204,6 +204,40 @@ int b2_stream_wait(b2_kv* kv, int index, int32_t* tokens_host, int timeout_ms);
 int b2_batch_begin(b2_model* m, b2_kv* kv, int B, void* stream);
 int b2_batch_set_row(b2_model* m, b2_kv* kv, int slot, int active, const b2_sampling* sampling, int first_token, void* stream);
 
+/* Beam search (generate(num_beams > 1): HF GenerationMixin._beam_search of the installed transformers 5.5, as the reference's eval
+ * scripts call it with --num_beams, llava/eval/run_llava.py:121,153). The B*nb running beams of B samples live in cache slots;
+ * the host (llava/_b2/beam.py) keeps the beam -> slot map and decides which slot becomes a copy of which after every step.
+ *   b2_kv_copy_slots   for each i, rows [row_begin, len(src_host[i])) of every layer's K and V (bytes and fp32 scales on an e4m3
+ *                      cache) are copied from slot src_host[i] to slot dst_host[i], and len(dst) := len(src). Rows below
+ *                      row_begin of dst are not touched. -1 when a dst is also a src of the call, a dst repeats, a slot is out
+ *                      of range or row_begin > len(src).
+ *   b2_op_beam_topk    per sample b, the K best continuations (score, token, beam) among nb beams x V tokens, where
+ *                      score = log_softmax(logits[row_of_beam[b*nb + j]]) + beam_scores[b*nb + j] in fp32 over the raw logits,
+ *                      sorted by score descending; equal scores go to the lower beam * V + token. NaN logits rank below -inf.
+ *                      row_of_beam (device int32 [B*nb]) may be NULL (= identity); beam_scores device fp32 [B*nb]; outputs
+ *                      device [B, K] (beam = index within the sample). nb <= 32, K <= 128, K <= nb * V.
+ *   b2_beam_step       one step of the running beams: the copies, then tokens_host[i] is fed to slot slot_of_beam_host[i]
+ *                      (every slot [0, B*nb) of the cache must hold one beam), one decode step at batch B*nb (the same path
+ *                      b2_decode_step takes), then b2_op_beam_topk over its logits with row_of_beam = slot_of_beam_host and
+ *                      the running scores, candidates written to the host arrays; returns after one stream synchronisation. */
+typedef struct b2_beam_step_args {
+    const int32_t* copy_src_host;     /* [n_copies] */
+    const int32_t* copy_dst_host;     /* [n_copies] */
+    int32_t n_copies;
+    int32_t row_begin;                /* first cache row the copies move (rows below are shared, e.g. the prompt) */
+    int32_t B, nb, K;
+    const int32_t* tokens_host;       /* [B*nb] token fed to running beam i (sample i / nb) */
+    const int32_t* slot_of_beam_host; /* [B*nb] cache slot of running beam i (after the copies) */
+    const float* beam_scores_host;    /* [B*nb] running score of beam i */
+    float* out_scores_host;           /* [B*K] */
+    int32_t* out_tokens_host;         /* [B*K] */
+    int32_t* out_beams_host;          /* [B*K] beam index within the sample */
+} b2_beam_step_args;
+int b2_kv_copy_slots(b2_model* m, b2_kv* kv, const int32_t* src_host, const int32_t* dst_host, int n, int row_begin, void* stream);
+int b2_op_beam_topk(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
+                    float* out_scores, int32_t* out_tokens, int32_t* out_beams, void* stream);
+int b2_beam_step(b2_model* m, b2_kv* kv, const b2_beam_step_args* args, void* stream);
+
 /* ---- single-kernel entry points (unit-level parity tests; same kernels the hot path launches) ----------- */
 int b2_op_gemm(const void* A, int lda, const void* W, int ldw, const void* bias, const void* residual, int ld_res,
                void* out, int ld_out, int out_fp32, int M, int N, int K, int act, int bn_override, void* stream);

@@ -1,0 +1,256 @@
+// Beam search on the device (generate(num_beams > 1), llava/_b2/beam.py holds the host half):
+//
+//   * beam_topk: per sample, the K best continuations among its nb beams x V tokens of
+//     score = log_softmax(logits[row_of_beam[beam]]) + beam_scores[beam] (fp32, torch's rounding order: (x - max) - log(sum)),
+//     sorted by score descending; ties go to the lower flat index beam * V + token. NaN logits are never preferred to a
+//     number (they rank below -inf); -inf is an ordinary value. Two launches: one CTA per beam row stages the row in shared
+//     memory, turns it into scores in place, radix-selects the row's K-th best key and compacts the row's top K in index
+//     order; a second launch merges the nb sorted lists of each sample by rank (binary search in every list).
+//     A candidate is one 64-bit key: order_key(score) << 32 | ~flat, so "larger key" is exactly the ranking rule above.
+//   * kv_copy_slots: cache slot dst := rows [row_begin, end) of slot src for every layer, head, K and V (and the fp32 scale
+//     rows of an e4m3 cache); one (layer, head, K|V) slab of one slot is contiguous, so each CTA streams 64 rows with
+//     16-byte vectors. The caller guarantees that no dst is also a src (b2_kv_copy_slots checks it), so pairs are independent.
+#include <limits.h>
+#include <math.h>
+
+#include "common.cuh"
+#include "kernels.h"
+
+namespace b2 {
+namespace {
+
+constexpr int BT_THREADS = 1024;
+constexpr int BM_THREADS = 256;
+constexpr int CP_THREADS = 256;
+constexpr int CP_ROWS = 64;  // cache rows per copy CTA (16 KiB of a bf16 slab)
+
+__device__ __forceinline__ uint32_t order_key(float x) {  // monotone float -> uint; NaN -> 0 (below -inf)
+    if (x != x) return 0u;
+    const uint32_t u = __float_as_uint(x);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float key_float(uint32_t k) {
+    return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k);
+}
+
+// fixed-order block reduction (warp shuffle tree, then the warp partials in order): the same bits on every run
+template <bool MAX>
+__device__ __forceinline__ float block_reduce(float v, float* s_w, int tid) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float w = __shfl_xor_sync(0xffffffffu, v, o);
+        v = MAX ? fmaxf(v, w) : v + w;
+    }
+    __syncthreads();
+    if ((tid & 31) == 0) s_w[tid >> 5] = v;
+    __syncthreads();
+    float t = s_w[0];
+    for (int i = 1; i < BT_THREADS / 32; ++i) t = MAX ? fmaxf(t, s_w[i]) : t + s_w[i];
+    return t;
+}
+
+__global__ void __launch_bounds__(BT_THREADS, 1)
+beam_row_topk_kernel(const float* __restrict__ logits, const int32_t* __restrict__ row_of_beam, const float* __restrict__ beam_scores,
+                     int nb, int V, int K, unsigned long long* __restrict__ keys_out) {
+    extern __shared__ __align__(16) uint8_t bt_smem[];
+    float* s_x = reinterpret_cast<float*>(bt_smem);
+    __shared__ float s_w[BT_THREADS / 32];
+    __shared__ int s_wa[BT_THREADS / 32];
+    __shared__ int s_gt;
+    __shared__ unsigned int s_hist[256];
+    __shared__ uint32_t s_prefix;
+    __shared__ int s_above;
+    __shared__ unsigned long long s_cand[128];
+
+    const int tid = threadIdx.x, j = blockIdx.x, b = blockIdx.y;
+    const int beam = b * nb + j;
+    const int row = row_of_beam ? row_of_beam[beam] : beam;
+    const float* x = logits + (size_t)row * V;
+    const int Kr = K < V ? K : V;  // candidates this row can supply
+
+    float mx = -INFINITY;
+    for (int i = tid; i < V; i += BT_THREADS) {
+        const float v = x[i];
+        s_x[i] = v;
+        if (v > mx) mx = v;  // NaN never compares greater
+    }
+    mx = block_reduce<true>(mx, s_w, tid);
+    float part = 0.f;
+    for (int i = tid; i < V; i += BT_THREADS) {
+        const float v = s_x[i];
+        if (v == v) part += expf(v - mx);
+    }
+    const float lse = logf(block_reduce<false>(part, s_w, tid));
+    const float run = beam_scores[beam];
+    for (int i = tid; i < V; i += BT_THREADS) s_x[i] = ((s_x[i] - mx) - lse) + run;
+    __syncthreads();
+
+    // radix descent for the key of the Kr-th largest score (8 bits per level from the top)
+    if (tid == 0) { s_prefix = 0u; s_above = 0; }
+    for (int level = 0; level < 4; ++level) {
+        const int shift = 24 - 8 * level;
+        if (tid < 256) s_hist[tid] = 0u;
+        __syncthreads();
+        const uint32_t prefix = s_prefix;
+        // log-probabilities crowd into a few digits (at level 0 nearly all share sign and exponent): one shared atomic per
+        // distinct digit of a warp instead of one per element, or the adds to the crowded bin serialise
+        for (int base = 0; base < V; base += BT_THREADS) {
+            const int i = base + tid;
+            const uint32_t key = i < V ? order_key(s_x[i]) : 0u;
+            const bool take = i < V && (level == 0 || (key >> (shift + 8)) == prefix);
+            const uint32_t digit = take ? ((key >> shift) & 255u) : 256u;
+            const unsigned peers = __match_any_sync(0xffffffffu, digit);
+            if (take && (tid & 31) == __ffs(peers) - 1) atomicAdd(&s_hist[digit], (unsigned)__popc(peers));
+        }
+        __syncthreads();
+        if (tid == 0) {
+            int acc = s_above, pick = 0;
+            for (int d = 255; d >= 0; --d) {
+                if (acc + (int)s_hist[d] >= Kr) { pick = d; break; }
+                acc += (int)s_hist[d];
+            }
+            s_above = acc;
+            s_prefix = (prefix << 8) | (uint32_t)pick;
+        }
+        __syncthreads();
+    }
+    const uint32_t kth = s_prefix;
+
+    // compaction in index order, 1024 consecutive elements per pass (a warp reads 32 consecutive words: no bank conflicts):
+    // every element above kth (their order does not matter, the rank sort below orders them), then the lowest-index elements
+    // equal to kth until Kr are taken. s_above now counts the elements above kth.
+    const int n_gt = s_above, need_eq = Kr - n_gt;
+    const unsigned long long flat0 = (unsigned long long)j * V;
+    const int lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) s_gt = 0;
+    __syncthreads();
+    int eq_seen = 0;  // uniform: elements equal to kth in the passes before this one
+    for (int base = 0; base < V; base += BT_THREADS) {
+        const int i = base + tid;
+        const uint32_t key = i < V ? order_key(s_x[i]) : 0u;
+        const unsigned long long cand = ((unsigned long long)key << 32) | (uint32_t)(0xFFFFFFFFu - (uint32_t)(flat0 + i));
+        if (i < V && key > kth) s_cand[atomicAdd(&s_gt, 1)] = cand;
+        const bool eq = i < V && key == kth;
+        const unsigned bal = __ballot_sync(0xffffffffu, eq);
+        if (lane == 0) s_wa[warp] = __popc(bal);
+        __syncthreads();
+        int before = 0, total = 0;
+        for (int w = 0; w < BT_THREADS / 32; ++w) {
+            before += w < warp ? s_wa[w] : 0;
+            total += s_wa[w];
+        }
+        if (eq) {
+            const int r = eq_seen + before + __popc(bal & ((1u << lane) - 1u));
+            if (r < need_eq) s_cand[n_gt + r] = cand;
+        }
+        eq_seen += total;
+        __syncthreads();
+        if (eq_seen >= need_eq && s_gt == n_gt) break;  // uniform: both parts complete
+    }
+    // sort the row's Kr candidates (descending key) by rank; pad the list with 0 (below every real candidate)
+    unsigned long long* out = keys_out + (size_t)beam * K;
+    if (tid < Kr) {
+        const unsigned long long me = s_cand[tid];
+        int rank = 0;
+        for (int c = 0; c < Kr; ++c) rank += s_cand[c] > me;
+        out[rank] = me;
+    } else if (tid < K) {
+        out[tid] = 0ull;
+    }
+}
+
+__global__ void __launch_bounds__(BM_THREADS)
+beam_merge_kernel(const unsigned long long* __restrict__ keys, int nb, int K, int V, float* __restrict__ out_scores,
+                  int32_t* __restrict__ out_tokens, int32_t* __restrict__ out_beams) {
+    const int b = blockIdx.x;
+    const unsigned long long* lists = keys + (size_t)b * nb * K;
+    for (int c = threadIdx.x; c < nb * K; c += BM_THREADS) {
+        const unsigned long long me = lists[c];
+        if (me == 0ull) continue;
+        int rank = 0;
+        for (int r = 0; r < nb && rank < K; ++r) {  // elements of sorted list r above me: binary search
+            const unsigned long long* l = lists + (size_t)r * K;
+            int a = 0, z = K;
+            while (a < z) {
+                const int mid = (a + z) >> 1;
+                if (l[mid] > me) a = mid + 1; else z = mid;
+            }
+            rank += a;
+        }
+        if (rank < K) {
+            const uint32_t flat = 0xFFFFFFFFu - (uint32_t)(me & 0xFFFFFFFFull);
+            out_scores[(size_t)b * K + rank] = key_float((uint32_t)(me >> 32));
+            out_tokens[(size_t)b * K + rank] = (int32_t)(flat % (uint32_t)V);
+            out_beams[(size_t)b * K + rank] = (int32_t)(flat / (uint32_t)V);
+        }
+    }
+}
+
+__global__ void __launch_bounds__(CP_THREADS)
+kv_copy_slots_kernel(uint8_t* __restrict__ k, uint8_t* __restrict__ v, float* __restrict__ ks, float* __restrict__ vs, KvCopyPairs p,
+                     int row_begin, int H, int max_batch, int pitch, int row_bytes, int32_t* __restrict__ len_dev) {
+    const int pair = blockIdx.z, lh = blockIdx.y >> 1, is_v = blockIdx.y & 1;
+    const int l = lh / H, h = lh % H;
+    const int src = p.src[pair], dst = p.dst[pair], end = p.end[pair];
+    if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) len_dev[dst] = end;
+    const int r0 = row_begin + blockIdx.x * CP_ROWS;
+    const int r1 = min(r0 + CP_ROWS, end);
+    if (r0 >= r1) return;
+    const size_t slab_src = ((size_t)l * max_batch + src) * H + h, slab_dst = ((size_t)l * max_batch + dst) * H + h;
+    uint8_t* base = is_v ? v : k;
+    const uint4* from = reinterpret_cast<const uint4*>(base + (slab_src * pitch + r0) * row_bytes);
+    uint4* to = reinterpret_cast<uint4*>(base + (slab_dst * pitch + r0) * row_bytes);
+    const int n16 = (r1 - r0) * row_bytes / 16;
+    for (int i = threadIdx.x; i < n16; i += CP_THREADS) to[i] = from[i];
+    if (ks != nullptr) {
+        float* sc = is_v ? vs : ks;
+        for (int i = threadIdx.x; i < r1 - r0; i += CP_THREADS) sc[slab_dst * pitch + r0 + i] = sc[slab_src * pitch + r0 + i];
+    }
+}
+
+}  // namespace
+
+size_t beam_topk_workspace_bytes(int B, int nb, int K) { return (size_t)B * nb * K * sizeof(unsigned long long); }
+
+int beam_topk(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
+              void* workspace, float* out_scores, int32_t* out_tokens, int32_t* out_beams, cudaStream_t stream) {
+    B2_CHECK_ARG(logits && beam_scores && workspace && out_scores && out_tokens && out_beams, "beam_topk: null argument");
+    B2_CHECK_ARG(B >= 1 && nb >= 1 && nb <= 32, "beam_topk: B=%d nb=%d (1 <= nb <= 32)", B, nb);
+    B2_CHECK_ARG(K >= 1 && K <= 128 && (long long)K <= (long long)nb * V, "beam_topk: K=%d outside [1, min(128, nb*V=%lld)]", K,
+                 (long long)nb * V);
+    const size_t smem = (size_t)V * sizeof(float);
+    B2_CHECK_ARG(V >= 1 && smem <= 200 * 1024 && (long long)nb * V < 0xFFFFFFFFll,
+                 "beam_topk: vocab %d exceeds the shared-memory staging of the kernel", V);
+    static size_t attr = 0;
+    if (smem > attr) {
+        B2_CUDA_CHECK(cudaFuncSetAttribute(beam_row_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attr = smem;
+    }
+    auto* keys = reinterpret_cast<unsigned long long*>(workspace);
+    beam_row_topk_kernel<<<dim3(nb, B), BT_THREADS, smem, stream>>>(logits, row_of_beam, beam_scores, nb, V, K, keys);
+    B2_LAUNCH_CHECK();
+    beam_merge_kernel<<<B, BM_THREADS, 0, stream>>>(keys, nb, K, V, out_scores, out_tokens, out_beams);
+    B2_LAUNCH_CHECK();
+    return 0;
+}
+
+int kv_copy_slots(void* k, void* v, float* kscale, float* vscale, const int32_t* src, const int32_t* dst, const int32_t* end, int n,
+                  int row_begin, int L, int H, int max_batch, int pitch, int row_bytes, int32_t* len_dev, cudaStream_t stream) {
+    B2_CHECK_ARG(row_bytes % 16 == 0 && row_begin >= 0, "kv_copy_slots: bad layout");
+    for (int off = 0; off < n; off += KvCopyPairs::kMax) {
+        const int c = n - off < KvCopyPairs::kMax ? n - off : KvCopyPairs::kMax;
+        KvCopyPairs p;
+        int rows = 1;
+        for (int i = 0; i < c; ++i) {
+            p.src[i] = src[off + i]; p.dst[i] = dst[off + i]; p.end[i] = end[off + i];
+            rows = end[off + i] - row_begin > rows ? end[off + i] - row_begin : rows;
+        }
+        const dim3 grid((rows + CP_ROWS - 1) / CP_ROWS, L * H * 2, c);
+        kv_copy_slots_kernel<<<grid, CP_THREADS, 0, stream>>>(reinterpret_cast<uint8_t*>(k), reinterpret_cast<uint8_t*>(v), kscale, vscale,
+                                                               p, row_begin, H, max_batch, pitch, row_bytes, len_dev);
+        B2_LAUNCH_CHECK();
+    }
+    return 0;
+}
+
+}  // namespace b2

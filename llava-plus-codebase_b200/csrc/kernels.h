@@ -227,6 +227,23 @@ int sample_publish(const float* logits, int V, int B, SampleState* st_dev, RowSt
                    cudaStream_t stream);
 int row_state_set(RowState* row_dev, const RowState& v, int32_t* tok_dev, int token, cudaStream_t stream);
 
+// ---- beam search (beam.cu) ---------------------------------------------------------------------------------------------------
+// per sample b, the K best (score, token, beam) of score = log_softmax(logits[row_of_beam[b*nb + j]]) + beam_scores[b*nb + j]
+// over its nb beams x V tokens, sorted by score descending, ties to the lower beam * V + token; row_of_beam null = identity.
+// nb <= 32, K <= min(128, nb * V); workspace >= beam_topk_workspace_bytes(B, nb, K)
+size_t beam_topk_workspace_bytes(int B, int nb, int K);
+int beam_topk(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
+              void* workspace, float* out_scores, int32_t* out_tokens, int32_t* out_beams, cudaStream_t stream);
+struct KvCopyPairs {
+    static constexpr int kMax = 64;
+    int32_t src[kMax], dst[kMax], end[kMax];
+};
+// for each pair i: rows [row_begin, end[i]) of cache slot src[i] -> slot dst[i], every layer / head / K and V (k / v bases of
+// [L][max_batch][H][pitch][row_bytes] bytes; kscale / vscale [L][max_batch][H][pitch] fp32 or null), and len_dev[dst[i]] = end[i].
+// No dst may be a src of the same call.
+int kv_copy_slots(void* k, void* v, float* kscale, float* vscale, const int32_t* src, const int32_t* dst, const int32_t* end, int n,
+                  int row_begin, int L, int H, int max_batch, int pitch, int row_bytes, int32_t* len_dev, cudaStream_t stream);
+
 // ---- image preprocessing (preprocess.cu): uint8 HWC -> CLIP pixel_values, PIL-exact bicubic resize ------------------------
 struct PreprocessArgs {
     const uint8_t* img = nullptr; int H = 0, W = 0;        // device, RGB HWC

@@ -152,6 +152,9 @@ struct b2_kv {
     int stream_B = 0, stream_tag = 0, stream_scheduled = 0;  // streaming generation in progress: tokens scheduled so far
     DevBuf rows_dev;               // RowState[max_batch] (continuous batching)
     std::vector<RowState> rows_host;
+    // b2_beam_step (allocated by the first call): beam -> slot map and running scores [2][max_batch], the per-row candidate
+    // keys of beam_topk, and its [B, K] outputs (scores, tokens, beams)
+    DevBuf beam_in, beam_ws, beam_out;
     bool e4m3() const { return dtype == B2_KV_E4M3; }
     size_t elem_bytes() const { return e4m3() ? 1 : 2; }
     size_t layer_rows() const { return (size_t)max_batch * m->d.heads * pitch; }  // = the layer stride of the scale arrays
@@ -786,7 +789,7 @@ int b2_init(int device) {
 }
 
 const char* b2_last_error(void) { return g_err; }
-int b2_version(void) { return 3; }
+int b2_version(void) { return 4; }
 unsigned long long b2_launch_count(void) { return g_launch_count; }
 
 int b2_model_create(const b2_model_desc* desc, b2_model** out) {
@@ -1151,7 +1154,8 @@ int b2_kv_destroy(b2_kv* kv) {
     if (kv->ev_fork) cudaEventDestroy(kv->ev_fork);
     if (kv->ev_join) cudaEventDestroy(kv->ev_join);
     DevBuf* bs[] = {&kv->k, &kv->v, &kv->kscale, &kv->vscale, &kv->len_dev, &kv->tok, &kv->step_counter, &kv->out_tokens, &kv->attn_partial,
-                    &kv->attn_counters, &kv->mega_layers, &kv->mega_sync, &kv->sk_partial, &kv->sk_counters, &kv->sstate, &kv->rows_dev, &kv->rope_tab};
+                    &kv->attn_counters, &kv->mega_layers, &kv->mega_sync, &kv->sk_partial, &kv->sk_counters, &kv->sstate, &kv->rows_dev, &kv->rope_tab,
+                    &kv->beam_in, &kv->beam_ws, &kv->beam_out};
     for (DevBuf* b : bs) b->free();
     delete kv;
     return 0;
@@ -1469,6 +1473,115 @@ int b2_decode_greedy(b2_model* m, b2_kv* kv, const int32_t* first_tokens, int B,
     B2_TRY(ws_leave(m, st));
     // a device destination stays asynchronous on the caller's stream; a host destination must be complete on return
     if (!is_device_pointer(out_tokens)) B2_CUDA_CHECK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+// ---- beam search: slot copies, candidate selection, one step of the running beams --------------------------------------
+// Checks a copy list against the cache (no side effects); end[i] = current length of src[i].
+static int check_copies(b2_kv* kv, const int32_t* src, const int32_t* dst, int n, int row_begin, std::vector<int32_t>& end) {
+    B2_CHECK_ARG(n >= 0 && n <= kv->max_batch && (n == 0 || (src != nullptr && dst != nullptr)) && row_begin >= 0,
+                 "b2_kv_copy_slots: bad argument (n=%d row_begin=%d)", n, row_begin);
+    std::vector<char> is_src(kv->max_batch, 0), is_dst(kv->max_batch, 0);
+    end.assign(n, 0);
+    for (int i = 0; i < n; ++i) {
+        B2_CHECK_ARG(src[i] >= 0 && src[i] < kv->max_batch && dst[i] >= 0 && dst[i] < kv->max_batch,
+                     "b2_kv_copy_slots: pair %d (%d -> %d) outside the cache's %d slots", i, src[i], dst[i], kv->max_batch);
+        B2_CHECK_ARG(row_begin <= kv->len_host[src[i]], "b2_kv_copy_slots: row_begin %d beyond the length %d of slot %d", row_begin,
+                     kv->len_host[src[i]], src[i]);
+        is_src[src[i]] = 1;
+        end[i] = kv->len_host[src[i]];
+    }
+    for (int i = 0; i < n; ++i) {
+        B2_CHECK_ARG(!is_dst[dst[i]], "b2_kv_copy_slots: slot %d is the destination of two copies", dst[i]);
+        B2_CHECK_ARG(!is_src[dst[i]], "b2_kv_copy_slots: slot %d is both a source and a destination", dst[i]);
+        is_dst[dst[i]] = 1;
+    }
+    return 0;
+}
+
+static int launch_copies(b2_model* m, b2_kv* kv, const int32_t* src, const int32_t* dst, const std::vector<int32_t>& end, int n,
+                         int row_begin, cudaStream_t st) {
+    if (n == 0) return 0;
+    B2_TRY(kv_copy_slots(kv->k.p, kv->v.p, kv->e4m3() ? kv->kscale.as<float>() : nullptr, kv->e4m3() ? kv->vscale.as<float>() : nullptr,
+                         src, dst, end.data(), n, row_begin, m->d.layers, m->d.heads, kv->max_batch, kv->pitch,
+                         (int)(m->hd * kv->elem_bytes()), kv->len_dev.as<int32_t>(), st));
+    for (int i = 0; i < n; ++i) kv->len_host[dst[i]] = end[i];
+    return 0;
+}
+
+int b2_kv_copy_slots(b2_model* m, b2_kv* kv, const int32_t* src_host, const int32_t* dst_host, int n, int row_begin, void* stream) {
+    B2_CHECK_ARG(m && kv && kv->m == m, "b2_kv_copy_slots: bad handle");
+    std::lock_guard<std::mutex> lk(m->mu);
+    DeviceGuard dg(m->device);
+    std::vector<int32_t> end;
+    B2_TRY(check_copies(kv, src_host, dst_host, n, row_begin, end));
+    return launch_copies(m, kv, src_host, dst_host, end, n, row_begin, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2_op_beam_topk(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
+                    float* out_scores, int32_t* out_tokens, int32_t* out_beams, void* stream) {
+    B2_CHECK_ARG(B >= 1 && nb >= 1 && nb <= 32 && K >= 1 && K <= 128, "b2_op_beam_topk: B=%d nb=%d K=%d", B, nb, K);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    void* ws = nullptr;
+    B2_CUDA_CHECK(cudaMallocAsync(&ws, beam_topk_workspace_bytes(B, nb, K), st));
+    const int r = beam_topk(logits, row_of_beam, beam_scores, B, nb, V, K, ws, out_scores, out_tokens, out_beams, st);
+    B2_CUDA_CHECK(cudaFreeAsync(ws, st));
+    return r;
+}
+
+int b2_beam_step(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, void* stream) {
+    B2_CHECK_ARG(m && kv && a && kv->m == m, "b2_beam_step: bad handle");
+    B2_CHECK_ARG(m->finalized, "b2_beam_step: model not finalized");
+    const int B = a->B, nb = a->nb, K = a->K, n = a->B * a->nb;
+    B2_CHECK_ARG(B >= 1 && nb >= 1 && nb <= 32 && n <= kv->max_batch, "b2_beam_step: B=%d x nb=%d beams exceed the cache's %d slots",
+                 B, nb, kv->max_batch);
+    B2_CHECK_ARG(K >= 1 && K <= 128 && (long long)K <= (long long)nb * m->d.vocab, "b2_beam_step: K=%d outside [1, min(128, nb*V)]", K);
+    B2_CHECK_ARG(a->tokens_host && a->slot_of_beam_host && a->beam_scores_host && a->out_scores_host && a->out_tokens_host &&
+                 a->out_beams_host, "b2_beam_step: null array");
+    std::lock_guard<std::mutex> lk(m->mu);
+    DeviceGuard dg(m->device);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    std::vector<int32_t> end;
+    B2_TRY(check_copies(kv, a->copy_src_host, a->copy_dst_host, a->n_copies, a->row_begin, end));
+    std::vector<int32_t> len(kv->len_host.begin(), kv->len_host.begin() + n), tok(n, -1);
+    for (int i = 0; i < a->n_copies; ++i)
+        if (a->copy_dst_host[i] < n) len[a->copy_dst_host[i]] = end[i];
+    for (int i = 0; i < n; ++i) {
+        const int s = a->slot_of_beam_host[i];
+        B2_CHECK_ARG(s >= 0 && s < n && tok[s] < 0, "b2_beam_step: slot_of_beam is not a permutation of [0, %d)", n);
+        B2_CHECK_ARG(a->tokens_host[i] >= 0, "b2_beam_step: negative token %d for beam %d", a->tokens_host[i], i);
+        tok[s] = a->tokens_host[i];
+    }
+    for (int s = 0; s < n; ++s)
+        B2_CHECK_ARG(len[s] >= 1 && len[s] < kv->max_seq, "b2_beam_step: slot %d has cache length %d (capacity %d)", s, len[s],
+                     kv->max_seq);
+    if (kv->beam_in.p == nullptr) {
+        B2_TRY(kv->beam_in.alloc((size_t)2 * kv->max_batch * 4));
+        B2_TRY(kv->beam_ws.alloc(beam_topk_workspace_bytes(kv->max_batch, 1, 128)));
+        B2_TRY(kv->beam_out.alloc((size_t)kv->max_batch * 128 * 12));
+    }
+    B2_TRY(ws_enter(m, st));
+    B2_TRY(launch_copies(m, kv, a->copy_src_host, a->copy_dst_host, end, a->n_copies, a->row_begin, st));
+    B2_TRY(copy_tokens_in(kv, tok.data(), n, st));
+    B2_CUDA_CHECK(cudaMemsetAsync(kv->step_counter.p, 0, 4, st));
+    B2_TRY(set_greedy_unpublished(kv, st));
+    cudaStream_t run = nullptr;
+    B2_TRY(fork_stream(kv, st, &run));
+    B2_TRY(decode_step_run(m, kv, n, run));
+    B2_TRY(join_stream(kv, st, run));
+    for (int s = 0; s < n; ++s) kv->len_host[s]++;
+    int32_t* rows = kv->beam_in.as<int32_t>();
+    B2_TRY(set_i32_pairs(rows, a->slot_of_beam_host, rows + kv->max_batch, reinterpret_cast<const int32_t*>(a->beam_scores_host), n, st));
+    float* o_s = kv->beam_out.as<float>();
+    int32_t* o_t = reinterpret_cast<int32_t*>(o_s + B * K);
+    int32_t* o_b = o_t + B * K;
+    B2_TRY(beam_topk(m->logits.as<float>(), rows, reinterpret_cast<const float*>(rows + kv->max_batch), B, nb, m->d.vocab, K, kv->beam_ws.p,
+                     o_s, o_t, o_b, st));
+    B2_CUDA_CHECK(cudaMemcpyAsync(a->out_scores_host, o_s, (size_t)B * K * 4, cudaMemcpyDeviceToHost, st));
+    B2_CUDA_CHECK(cudaMemcpyAsync(a->out_tokens_host, o_t, (size_t)B * K * 4, cudaMemcpyDeviceToHost, st));
+    B2_CUDA_CHECK(cudaMemcpyAsync(a->out_beams_host, o_b, (size_t)B * K * 4, cudaMemcpyDeviceToHost, st));
+    B2_TRY(ws_leave(m, st));
+    B2_CUDA_CHECK(cudaStreamSynchronize(st));
     return 0;
 }
 

@@ -55,6 +55,13 @@ class PreprocessPlan(_c.Structure):
                 ("pixels", _vp), ("u8_out", _vp)]
 
 
+class BeamStepArgs(_c.Structure):
+    """b2_beam_step_args (include/b2llava.h)."""
+    _fields_ = [("copy_src_host", _vp), ("copy_dst_host", _vp), ("n_copies", _c.c_int32), ("row_begin", _c.c_int32),
+                ("B", _c.c_int32), ("nb", _c.c_int32), ("K", _c.c_int32), ("tokens_host", _vp), ("slot_of_beam_host", _vp),
+                ("beam_scores_host", _vp), ("out_scores_host", _vp), ("out_tokens_host", _vp), ("out_beams_host", _vp)]
+
+
 def make_sampling(do_sample=False, temperature=1.0, top_p=1.0, top_k=0, seed=0):
     return Sampling(int(bool(do_sample)), float(temperature), float(1.0 if top_p is None else top_p),
                     int(top_k or 0), int(seed) & (2**64 - 1))
@@ -97,6 +104,9 @@ SIGNATURES = {
     "b2_decode_step": (_i32, [_vp, _vp, _vp, _i32, _vp, _vp, _vp]),
     "b2_decode_greedy": (_i32, [_vp, _vp, _vp, _i32, _i32, _vp, _vp]),
     "b2_argmax": (_i32, [_vp, _i32, _i32, _vp, _vp]),
+    "b2_kv_copy_slots": (_i32, [_vp, _vp, _c.POINTER(_c.c_int32), _c.POINTER(_c.c_int32), _i32, _i32, _vp]),
+    "b2_op_beam_topk": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
+    "b2_beam_step": (_i32, [_vp, _vp, _c.POINTER(BeamStepArgs), _vp]),
     "b2_op_gemm": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "b2_op_gemv": (_i32, [_vp, _i64, _vp, _i32, _vp, _f32, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "b2_op_gemm_skinny": (_i32, [_vp, _i32, _vp, _i32, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _vp]),
@@ -434,6 +444,51 @@ class Engine:
             check(self.lib.b2_op_sample(ptr(logits), B, V, ctypes.byref(sampling), int(index), ptr(out), stream_ptr()),
                   "b2_op_sample")
         return out
+
+    # -- beam search (generate(num_beams > 1); host half in llava/_b2/beam.py) ------------------------------------------------
+    def kv_copy_slots(self, kv, src, dst, row_begin=0):
+        """Rows [row_begin, len(src[i])) of slot src[i] -> slot dst[i], all layers; afterwards len(dst[i]) == len(src[i])."""
+        n = len(src)
+        if len(dst) != n:
+            raise ValueError(f"{n} sources for {len(dst)} destinations")
+        s, d = (_c.c_int32 * max(n, 1))(*src), (_c.c_int32 * max(n, 1))(*dst)
+        with torch.cuda.device(self.index):
+            check(self.lib.b2_kv_copy_slots(self.handle, kv.handle, s, d, n, int(row_begin), stream_ptr()), "b2_kv_copy_slots")
+
+    def beam_topk(self, logits, beam_scores, nb, K, row_of_beam=None):
+        """logits fp32 [rows, V] (device); beam_scores [B*nb]; row_of_beam int [B*nb] or None (identity). Returns device
+        tensors (scores fp32, tokens int32, beams int32), each [B, K], best first (b2_op_beam_topk)."""
+        V = logits.shape[-1]
+        scores = beam_scores.to(device=self.device, dtype=torch.float32).contiguous()
+        B = scores.numel() // nb
+        rows = None if row_of_beam is None else torch.as_tensor(row_of_beam, dtype=torch.int32).to(self.device).contiguous()
+        out_s = torch.empty(B, K, dtype=torch.float32, device=self.device)
+        out_t = torch.empty(B, K, dtype=torch.int32, device=self.device)
+        out_b = torch.empty(B, K, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.index):
+            check(self.lib.b2_op_beam_topk(ptr(logits), ptr(rows), ptr(scores), B, int(nb), V, int(K), ptr(out_s), ptr(out_t),
+                                           ptr(out_b), stream_ptr()), "b2_op_beam_topk")
+        return out_s, out_t, out_b
+
+    def beam_step(self, kv, copies, row_begin, tokens, slot_of_beam, beam_scores, nb, K):
+        """One step of the running beams (b2_beam_step): `copies` = [(src, dst)] applied first, tokens[i] fed to slot
+        slot_of_beam[i], one decode step at batch len(tokens), candidates of every sample selected on the device. Returns CPU
+        tensors (scores fp32, tokens int64, beams int64), each [B, K], best first."""
+        n = len(tokens)
+        B = n // nb
+        i32 = lambda xs: (_c.c_int32 * max(len(xs), 1))(*[int(x) for x in xs])
+        src, dst = i32([c[0] for c in copies]), i32([c[1] for c in copies])
+        toks, slots = i32(tokens), i32(slot_of_beam)
+        scores = (_c.c_float * n)(*[float(x) for x in beam_scores])
+        out_s = torch.empty(B, K, dtype=torch.float32)
+        out_t = torch.empty(B, K, dtype=torch.int32)
+        out_b = torch.empty(B, K, dtype=torch.int32)
+        a = BeamStepArgs(_c.cast(src, _vp), _c.cast(dst, _vp), len(copies), int(row_begin), B, int(nb), int(K), _c.cast(toks, _vp),
+                         _c.cast(slots, _vp), _c.cast(scores, _vp), _vp(out_s.data_ptr()), _vp(out_t.data_ptr()),
+                         _vp(out_b.data_ptr()))
+        with torch.cuda.device(self.index):
+            check(self.lib.b2_beam_step(self.handle, kv.handle, ctypes.byref(a), stream_ptr()), "b2_beam_step")
+        return out_s, out_t.long(), out_b.long()
 
     def argmax(self, logits):
         B, V = logits.shape

@@ -306,7 +306,7 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             hidden=c.hidden_size, inter=c.intermediate_size, layers=c.num_hidden_layers,
             heads=c.num_attention_heads, vocab=self.lm_head.weight.shape[0], rms_eps=c.rms_norm_eps,
             rope_theta=float(getattr(c, "rope_theta", None) or (getattr(c, "rope_parameters", None) or {}).get("rope_theta", 10000.0)),
-            max_batch=max(self._limits["max_batch"] or 1, int(getattr(c, "b2_continuous_batching", 0) or 0)),
+            max_batch=max(self._limits["max_batch"] or 1, int(getattr(c, "b2_continuous_batching", 0) or 0), self._beam_search_cap()),
             max_seq=max_seq, max_images=self._limits["max_images"] or 8,
         )
         if getattr(vc, "hidden_act", "quick_gelu") != "quick_gelu":
@@ -497,8 +497,12 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             inputs = input_ids
         if inputs is None:
             raise ValueError("generate() needs input ids")
+        beam_args = {}
         if num_beams != 1:
-            raise NotImplementedError("beam search is not used on the LLaVA path (num_beams=1 everywhere)")
+            if self._beam_search_cap() < 2:
+                raise NotImplementedError("beam search is not used on the LLaVA path (num_beams=1 everywhere)")
+            beam_args = self._beam_arguments(num_beams, do_sample, temperature, streamer, output_scores, return_dict_in_generate,
+                                             kwargs)
         if return_dict_in_generate or output_scores:
             raise NotImplementedError("generate() returns the id tensor only")
         for k, v in kwargs.items():
@@ -519,6 +523,11 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             max_new_tokens = (max_length - Lt) if max_length is not None else 20
         if max_new_tokens <= 0:
             raise ValueError("max_new_tokens must be positive")
+        if beam_args:
+            eos_list = (list(eos_token_id) if isinstance(eos_token_id, (list, tuple))
+                        else (None if eos_token_id is None else [eos_token_id]))
+            return self._beam_generate(engine, prompt, images, attention_mask, num_beams, max_new_tokens, eos_list, pad_token_id,
+                                       stopping_criteria, **beam_args)
         greedy = (not do_sample) or (temperature is not None and temperature <= 1e-5)
         if greedy:
             sampling = make_sampling()
@@ -573,19 +582,7 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         try:
             # ---- prefill: splice + decoder, last-position logits only; token 0 is chosen on the device ----
             def prefill(force_host):
-                embeds, lens, speculative = None, None, False
-                if images is not None and self.get_vision_tower() is not None:
-                    embeds, lens, speculative = self._spliced_embeds(prompt, attention_mask, images, force_host=force_host)
-                if embeds is not None:
-                    if getattr(self.config, "tokenizer_padding_side", "right") == "left" and len(set(lens)) > 1:
-                        S = embeds.shape[1]
-                        embeds = torch.stack([torch.roll(embeds[b], shifts=-(S - lens[b]), dims=0) for b in range(B)])
-                else:  # text-only prompt (or a [B,1] prompt, which the multimodal splice passes through)
-                    if attention_mask is not None and not bool(attention_mask.bool().all()):
-                        raise NotImplementedError("padded text-only batches: pass equal-length prompts")
-                    ids = prompt.to(torch.int32).reshape(-1).to(engine.device)
-                    embeds = engine.splice(ids, None, B, Lt)
-                    lens = [Lt] * B
+                embeds, lens, speculative = self._prompt_embeds(engine, prompt, attention_mask, images, force_host)
                 if prof: prof.mark("encode_images+splice")
                 self._check_limits(engine, B, max(lens) + max_new_tokens)
                 kv.reset()
@@ -627,6 +624,100 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         out = torch.cat([prompt, new_tokens.to(device=prompt.device, dtype=prompt.dtype)], dim=1)
         if prof: prof.mark("ids to caller"); prof.report()
         return out
+
+    def _prompt_embeds(self, engine, prompt, attention_mask, images, force_host):
+        """Spliced prompt rows of generate(): (embeds [B, S, hidden], valid rows per sample, whether the device splice was
+        used on the shape-only assumption that every row holds n_images / B placeholders)."""
+        B, Lt = prompt.shape
+        embeds, lens, speculative = None, None, False
+        if images is not None and self.get_vision_tower() is not None:
+            embeds, lens, speculative = self._spliced_embeds(prompt, attention_mask, images, force_host=force_host)
+        if embeds is not None:
+            if getattr(self.config, "tokenizer_padding_side", "right") == "left" and len(set(lens)) > 1:
+                S = embeds.shape[1]
+                embeds = torch.stack([torch.roll(embeds[b], shifts=-(S - lens[b]), dims=0) for b in range(B)])
+        else:  # text-only prompt (or a [B,1] prompt, which the multimodal splice passes through)
+            if attention_mask is not None and not bool(attention_mask.bool().all()):
+                raise NotImplementedError("padded text-only batches: pass equal-length prompts")
+            ids = prompt.to(torch.int32).reshape(-1).to(engine.device)
+            embeds = engine.splice(ids, None, B, Lt)
+            lens = [Lt] * B
+        return embeds, lens, speculative
+
+    # ------------------------------------------------------------------ beam search
+    def _beam_search_cap(self):
+        """config.b2_beam_search or B2_BEAM_SEARCH: the largest num_beams generate() accepts (beam search is off below 2). It
+        also sizes the engine's caches, like b2_continuous_batching."""
+        v = getattr(self.config, "b2_beam_search", None)
+        if v is None:
+            v = os.environ.get("B2_BEAM_SEARCH")
+        try:
+            return int(v or 0)
+        except (TypeError, ValueError):
+            raise ValueError(f"b2_beam_search must be an integer, got {v!r}")
+
+    def _beam_arguments(self, num_beams, do_sample, temperature, streamer, output_scores, return_dict_in_generate, kwargs):
+        """Checks what generate(num_beams > 1) does not implement and takes the beam-only arguments out of `kwargs`."""
+        if num_beams < 1 or num_beams > self._beam_search_cap():
+            raise ValueError(f"num_beams={num_beams} exceeds config.b2_beam_search={self._beam_search_cap()}")
+        if do_sample and not (temperature is not None and temperature <= 1e-5):
+            raise NotImplementedError("beam sampling (do_sample=True with num_beams > 1) is not implemented on the H100 path")
+        if (kwargs.get("num_beam_groups") or 1) != 1 or (kwargs.get("diversity_penalty") or 0.0) != 0.0:
+            raise NotImplementedError("group beam search (num_beam_groups / diversity_penalty) is not implemented on the H100 path")
+        if kwargs.get("constraints") is not None:
+            raise NotImplementedError("constrained beam search (constraints) is not implemented on the H100 path")
+        if output_scores or return_dict_in_generate:
+            raise NotImplementedError("beam search returns the id tensor only (output_scores / return_dict_in_generate)")
+        if streamer is not None:
+            raise ValueError("`streamer` cannot be used with beam search (num_beams > 1)")
+        lp = kwargs.pop("length_penalty", None)
+        es = kwargs.pop("early_stopping", None)
+        nrs = kwargs.pop("num_return_sequences", None)
+        return dict(length_penalty=1.0 if lp is None else float(lp), early_stopping=False if es is None else es,
+                    num_return_sequences=1 if nrs is None else int(nrs))
+
+    def _beam_generate(self, engine, prompt, images, attention_mask, num_beams, max_new_tokens, eos_ids, pad_token_id,
+                       stopping_criteria, length_penalty, early_stopping, num_return_sequences):
+        """Beam search (llava/_b2/beam.py): sample b is prefilled once into slot b of a pool cache; its candidates from the
+        prefill logits fork the prompt into nb slots; then every b2_beam_step applies the step's slot copies, decodes the
+        B * nb running beams in one batch and returns the K best candidates per sample for the host bookkeeping."""
+        from ..._b2 import beam as _beam
+
+        B = prompt.shape[0]
+        nb = num_beams
+        search = _beam.BeamSearch(prompt, nb, max_new_tokens, eos_ids, length_penalty, early_stopping, num_return_sequences,
+                                  pad_token_id, stopping_criteria)
+        if engine.vocab < search.K:
+            raise ValueError(f"beam search keeps {search.K} candidates per step, more than the vocabulary ({engine.vocab})")
+        self._check_limits(engine, B * nb, 1)
+        kv = self._pool.acquire()  # exclusive for this call; never recorded for prefix reuse
+        try:
+            def first_candidates(force_host):
+                embeds, lens, speculative = self._prompt_embeds(engine, prompt, attention_mask, images, force_host)
+                self._check_limits(engine, B * nb, max(lens) + max_new_tokens)
+                kv.reset()
+                logits = engine.prefill(kv, embeds, lens, LOGITS_LAST)
+                cand = [t.cpu() for t in engine.beam_topk(logits, torch.zeros(B), 1, search.K)]  # synchronises
+                return cand, lens, speculative
+
+            cand, lens, speculative = first_candidates(False)
+            err = engine.take_async_error()
+            if speculative and (err & ERR_SPLICE_SLOTS):
+                cand, lens, _ = first_candidates(True)
+                err = engine.take_async_error()
+            if err:
+                raise ValueError(last_error())
+            planner = _beam.SlotPlanner(B, nb)
+            row_begin = 0  # the first plan copies whole prompts; later ones only rows behind the shortest prompt
+            while not search.step(*cand):
+                copies = planner.plan(search.parents)
+                cand = engine.beam_step(kv, copies, row_begin, search.next_tokens().tolist(), planner.flat(),
+                                        search.running_scores.reshape(-1).tolist(), nb, search.K)
+                row_begin = min(lens)
+            engine.check_async_error()
+        finally:
+            self._pool.release(kv)
+        return search.output()[0].to(device=prompt.device, dtype=prompt.dtype)
 
     def _prefix_cache_on(self):
         """config.b2_prefix_cache or B2_PREFIX_CACHE=1 (off by default: logits of reused answer rows, which the decode kernels
