@@ -96,6 +96,18 @@ int b2_model_destroy(b2_model* m);
  * fp8 path; oracle/fp8_oracle.py defines the arithmetic and the tolerance (tests/test_fp8_gpu.py). Off unless this call is
  * made: it changes the numerics of the decode step (W8A8), so it is never a default. */
 int b2_model_enable_fp8_decode(b2_model* m);
+/* load_4bit (reference llava/model/builder.py:26-41, bitsandbytes NF4): after finalize, quantise the seven decoder Linears
+ * of every layer to NF4 (per row, one fp32 absmax per 64-element block, 4-bit codes into the NF4 table; oracle/nf4_oracle.py
+ * defines the arithmetic) and free their bf16 buffers; replace both mm_projector weights in place by their dequantised
+ * values w_hat = bf16(code * absmax). Decode at batch <= 8 then streams the 4-bit weights (gemv_nf4, whose activation tile
+ * must fit shared memory: 13B shapes at batch 5..8 do not); prefill and the other decode batches dequantise one layer at a
+ * time into a bf16 scratch and run the dense kernels over it. The CLIP tower,
+ * embed_tokens, lm_head and the norms stay bf16. Returns -1 when the model is not finalized, when
+ * b2_model_enable_fp8_decode has run, or when a KV cache of this model exists; a second call is a no-op. Afterwards
+ * b2_model_enable_fp8_decode and b2_model_set_weight on a decoder Linear or projector weight return -1. */
+int b2_model_enable_nf4(b2_model* m);
+/* device bytes of the weights the model holds (bf16, e4m3 and NF4 copies with their scales; workspaces excluded) */
+int64_t b2_model_weight_bytes(b2_model* m);
 
 int b2_kv_create(b2_model* m, int max_batch, int max_seq, b2_kv** out); /* KV cache [L][2][B][H][Smax][128] bf16 */
 /* b2_kv_create with the element format chosen per cache; b2_kv_create == kv_dtype B2_KV_BF16. B2_KV_E4M3 stores K and V as e4m3
@@ -244,6 +256,14 @@ int b2_op_gemm(const void* A, int lda, const void* W, int ldw, const void* bias,
 int b2_op_gemv(const void* x, int64_t ldx, const void* W, int ldw, const void* norm_gamma, float eps,
                const void* residual, int ld_res, void* out, int ld_out, int out_fp32, int B, int N, int K, int act,
                void* stream);
+/* NF4 (b2_model_enable_nf4). Canonical layout: codes [N, K/2] bytes, element 2j in the high nibble of byte j; absmax
+ * [N, K/64] fp32. quantize: w bf16 [N, K] contiguous, K % 64 == 0. dequantize: out bf16 [N, K] = w_hat. */
+int b2_op_quantize_nf4(const void* w, int N, int K, void* codes, float* absmax, void* stream);
+int b2_op_dequantize_nf4(const void* codes, const float* absmax, int N, int K, void* out, void* stream);
+/* b2_op_gemv over NF4 weights: codes in the GEMV order (oracle/nf4_oracle.py pack_nf4(order="gemv")), absmax [N, K/64];
+ * K % 128 == 0, bf16 output; out = (rmsnorm(x) | x) . w_hat^T (+ residual), or SwiGLU over block-64 interleaved rows. */
+int b2_op_gemv_nf4(const void* x, int64_t ldx, const void* codes, const float* absmax, const void* norm_gamma, float eps,
+                   const void* residual, int ld_res, void* out, int ld_out, int B, int N, int K, int act, void* stream);
 /* decode Linear at batch 9..128 (swap-AB stream-K wgmma GEMM, csrc/gemm_skinny.cu): out[B,N] = x[B,K]·W[N,K]^T
  * (+ residual); act = B2_ACT_NONE | B2_ACT_SWIGLU (out [B,N/2], W rows block-64 interleaved). `workspace` (fp32,
  * >= b2_op_gemm_skinny_workspace_bytes) and `counters` (int32, >= b2_op_gemm_skinny_counter_bytes, zero-filled once

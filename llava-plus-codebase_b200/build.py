@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libb2llava.so")
-SOURCES = ["gemm_wgmma.cu", "gemm_skinny.cu", "quant_fp8.cu", "gemv.cu", "decode_mega.cu", "attention.cu", "attention_wgmma.cu", "norms.cu", "vit_ops.cu", "misc_ops.cu", "sampling.cu", "beam.cu", "preprocess.cu", "model.cu"]
+SOURCES = ["gemm_wgmma.cu", "gemm_skinny.cu", "quant_fp8.cu", "gemv.cu", "decode_mega.cu", "attention.cu", "attention_wgmma.cu", "norms.cu", "vit_ops.cu", "misc_ops.cu", "sampling.cu", "beam.cu", "nf4.cu", "preprocess.cu", "model.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",

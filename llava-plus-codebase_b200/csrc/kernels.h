@@ -87,6 +87,21 @@ struct GemvArgs {
 int gemv_bf16(const GemvArgs& g, cudaStream_t stream);
 bool gemv_fits(int B, int N, int K, int act);  // activation tile + partial table fit in shared memory
 
+// ---- NF4 weights (nf4.cu; format in DESIGN.md §2-3) ------------------------------------------------------------
+// w bf16 [N, K] (row pitch ldw) -> codes [N, K/2] bytes + absmax [N, K/64] fp32; K % 64 == 0. gemv_order = 0: canonical
+// layout (element 2j in the high nibble of byte j); 1: the order gemv_nf4 reads (K % 128 == 0)
+int quantize_nf4(const void* w, int64_t ldw, int N, int K, void* q, float* absmax, int gemv_order, cudaStream_t stream);
+struct Nf4Matrix {
+    const void* q = nullptr; const float* absmax = nullptr;
+    void* out = nullptr;  // bf16 [N, K], contiguous
+    int N = 0, K = 0;
+};
+// w_hat = bf16(code * absmax) of up to four matrices in one launch
+int dequantize_nf4(const Nf4Matrix* mats, int n, int gemv_order, cudaStream_t stream);
+// gemv_bf16's contract over NF4 weights in GEMV order (g.W unused; bf16 output only); K % 128 == 0
+int gemv_nf4(const GemvArgs& g, const void* q, const float* absmax, cudaStream_t stream);
+bool gemv_nf4_fits(int B, int N, int K, int act);
+
 // ---- norms (norms.cu) ------------------------------------------------------------------------------
 int layernorm_bf16(const void* x, const void* gamma, const void* beta, void* y, int rows, int cols, float eps,
                    cudaStream_t stream);

@@ -9,6 +9,8 @@
 #include <string.h>
 #include <time.h>
 
+#include <atomic>
+#include <utility>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -70,6 +72,9 @@ struct LlamaLayer {
     unsigned qkv_parts = 0;
     DevBuf wqkv8, wo8, wgu8, wd8, s_qkv, s_o, s_gu, s_d;  // e4m3 copies + per-row fp32 scales (b2_model_enable_fp8_decode)
     DevBuf tmp_gate, tmp_up;  // staging until both halves arrived
+    // NF4 (b2_model_enable_nf4): codes in GEMV order [N, K/2] and absmax [N, K/64] of wqkv / wo / wgu / wd; the bf16 buffers
+    // above are freed
+    DevBuf q_qkv, a_qkv, q_o, a_o, q_gu, a_gu, q_d, a_d;
     bool has_gate = false, has_up = false;
 };
 }  // namespace
@@ -117,6 +122,11 @@ struct b2_model {
     // e4m3 KV caches: one layer of roped bf16 K / V, [B][H][S][128], that prefill attends over before it is quantised into
     // the cache (allocated with the first e4m3 cache)
     DevBuf kstage, vstage;
+    // NF4 decoder Linears (b2_model_enable_nf4): the dense kernels read one layer's w_hat from this bf16 scratch
+    // (wqkv | wo | wgu | wd, dequantised by one launch per layer); a workspace like the ones above
+    bool nf4 = false;
+    DevBuf nf4_scratch;
+    std::atomic<int> kv_live{0};  // KV caches created on this model and not destroyed
 };
 
 struct b2_kv {
@@ -155,6 +165,7 @@ struct b2_kv {
     // b2_beam_step (allocated by the first call): beam -> slot map and running scores [2][max_batch], the per-row candidate
     // keys of beam_topk, and its [B, K] outputs (scores, tokens, beams)
     DevBuf beam_in, beam_ws, beam_out;
+    bool counted = false;  // included in m->kv_live
     bool e4m3() const { return dtype == B2_KV_E4M3; }
     size_t elem_bytes() const { return e4m3() ? 1 : 2; }
     size_t layer_rows() const { return (size_t)max_batch * m->d.heads * pitch; }  // = the layer stride of the scale arrays
@@ -270,6 +281,41 @@ bool use_skinny(const b2_kv* kv, int B) {
     return !(e != nullptr && e[0] == '0');
 }
 
+// bf16 weights of decoder layer l for the dense kernels (wgmma tile GEMMs, stream-K GEMM): the ingested buffers, or on an NF4
+// model the layer's w_hat, dequantised into the model's one-layer scratch by one launch
+struct LayerW { const void *wqkv, *wo, *wgu, *wd; };
+int layer_weights(b2_model* m, int l, LayerW* w, cudaStream_t st) {
+    LlamaLayer& L = m->ll[l];
+    if (!m->nf4) { *w = {L.wqkv.p, L.wo.p, L.wgu.p, L.wd.p}; return 0; }
+    const int h = m->d.hidden, I = m->d.inter;
+    bf16* s = m->nf4_scratch.as<bf16>();
+    Nf4Matrix mt[4];
+    const DevBuf* q[4] = {&L.q_qkv, &L.q_o, &L.q_gu, &L.q_d};
+    const DevBuf* a[4] = {&L.a_qkv, &L.a_o, &L.a_gu, &L.a_d};
+    const int N[4] = {3 * h, h, 2 * I, h}, K[4] = {h, h, h, I};
+    bf16* out = s;
+    for (int i = 0; i < 4; ++i) {
+        mt[i].q = q[i]->p; mt[i].absmax = a[i]->as<float>(); mt[i].out = out; mt[i].N = N[i]; mt[i].K = K[i];
+        out += (size_t)N[i] * K[i];
+    }
+    B2_TRY(dequantize_nf4(mt, 4, 1, st));
+    *w = {mt[0].out, mt[1].out, mt[2].out, mt[3].out};
+    return 0;
+}
+// NF4 decode at batch <= 8: gemv_nf4 for the seven decoder Linears when every shape fits its shared-memory budget
+bool use_gemv_nf4(const b2_model* m, int B) {
+    const int h = m->d.hidden, I = m->d.inter;
+    return m->nf4 && B <= 8 && gemv_nf4_fits(B, 3 * h, h, ACT_NONE) && gemv_nf4_fits(B, h, h, ACT_NONE) &&
+           gemv_nf4_fits(B, 2 * I, h, ACT_SWIGLU) && gemv_nf4_fits(B, h, I, ACT_NONE);
+}
+int gemv4(const void* x, int64_t ldx, const DevBuf& q, const DevBuf& a, const void* gamma, float eps, const void* res, int ld_res,
+          void* out, int ld_out, int B, int N, int K, int act, cudaStream_t st) {
+    GemvArgs g;
+    g.x = x; g.ldx = ldx; g.norm_gamma = gamma; g.eps = eps; g.residual = res; g.ld_res = ld_res;
+    g.out = out; g.ld_out = ld_out; g.B = B; g.N = N; g.K = K; g.act = act;
+    return gemv_nf4(g, q.p, a.as<float>(), st);
+}
+
 int decode_nsplit(int B, int H, int max_seq, int ctas_per_sm) {
     // Split-KV factor of the multi-kernel decode step. The kernel is register-limited to `occ` resident CTAs per SM, so one wave
     // is occ*SMs CTAs. Few (batch, head) pairs: fill one wave; otherwise 3 splits (short enough ranges for the tail wave to
@@ -360,6 +406,10 @@ int set_llama_layer_weight(b2_model* m, int li, const std::string& s, const char
                            const int64_t* shape, int ndim, int dt) {
     const int h = m->d.hidden, I = m->d.inter;
     LlamaLayer& L = m->ll[li];
+    if (m->nf4 && (starts_with(s, "self_attn.") || starts_with(s, "mlp.")) && s != "self_attn.rotary_emb.inv_freq") {
+        set_error("set_weight(%s): the decoder Linears of this model are NF4 (b2_model_enable_nf4); they cannot be reloaded", key);
+        return -1;
+    }
     if (s == "input_layernorm.weight") { B2_TRY(expect_shape(key, shape, ndim, h)); return put(L.ln1, h, 0, ptr, dt, h); }
     if (s == "post_attention_layernorm.weight") { B2_TRY(expect_shape(key, shape, ndim, h)); return put(L.ln2, h, 0, ptr, dt, h); }
     const char* names[3] = {"self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight"};
@@ -513,13 +563,19 @@ int decode_step_launch(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     // batch <= 8: tensor-core GEMV kernels (falls back to the skinny-M wgmma GEMM when the activations do not fit smem)
     // batch 7..128: swap-AB stream-K GEMM (weights streamed once, all SMs busy); otherwise GEMV kernels (B <= 8) or
     // the tile GEMM
-    const bool sk = use_skinny(kv, B);
-    const bool small = !sk && B <= 8 && gemv_fits(B, h, I, ACT_NONE) && gemv_fits(B, 2 * I, h, ACT_SWIGLU) &&
+    // NF4 model: gemv_nf4 at batch <= 8; otherwise each layer is dequantised into the scratch in front of the paths below
+    const bool small4 = use_gemv_nf4(m, B);
+    const bool sk = !small4 && use_skinny(kv, B);
+    const bool small = !m->nf4 && !sk && B <= 8 && gemv_fits(B, h, I, ACT_NONE) && gemv_fits(B, 2 * I, h, ACT_SWIGLU) &&
                        gemv_fits(B, 3 * h, h, ACT_NONE) && gemv_fits(B, V, h, ACT_NONE);
     const bool f8 = sk && m->fp8_decode;  // e4m3 weights x e4m3 activations through the same stream-K GEMM
     for (int l = 0; l < d.layers; ++l) {
         LlamaLayer& L = m->ll[l];
-        if (f8) {
+        LayerW lw = {};
+        if (!small4) B2_TRY(layer_weights(m, l, &lw, st));
+        if (small4) {
+            B2_TRY(gemv4(m->x.p, h, L.q_qkv, L.a_qkv, L.ln1.p, d.rms_eps, nullptr, 0, m->qkv.p, 3 * h, B, 3 * h, h, ACT_NONE, st));
+        } else if (f8) {
             B2_TRY(rmsnorm_quant_e4m3(m->x.p, h, L.ln1.p, m->xq8.p, h, m->xscale.as<float>(), B, h, d.rms_eps, st));
             B2_TRY(skinny8(m, kv, L.wqkv8.p, L.s_qkv.as<float>(), nullptr, 0, m->qkv.p, 3 * h, 0, B, 3 * h, h, ACT_NONE, st));
         } else if (small) {
@@ -527,10 +583,10 @@ int decode_step_launch(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
                         ACT_NONE, st));
         } else if (sk) {
             B2_TRY(rmsnorm_bf16(m->x.p, h, L.ln1.p, m->xn.p, B, h, d.rms_eps, st));
-            B2_TRY(skinny(kv, m->xn.p, h, L.wqkv.p, h, nullptr, 0, m->qkv.p, 3 * h, 0, B, 3 * h, h, ACT_NONE, st));
+            B2_TRY(skinny(kv, m->xn.p, h, lw.wqkv, h, nullptr, 0, m->qkv.p, 3 * h, 0, B, 3 * h, h, ACT_NONE, st));
         } else {
             B2_TRY(rmsnorm_bf16(m->x.p, h, L.ln1.p, m->xn.p, B, h, d.rms_eps, st));
-            B2_TRY(gemm(m->xn.p, h, L.wqkv.p, h, nullptr, nullptr, 0, m->qkv.p, 3 * h, 0, B, 3 * h, h, ACT_NONE, st));
+            B2_TRY(gemm(m->xn.p, h, lw.wqkv, h, nullptr, nullptr, 0, m->qkv.p, 3 * h, 0, B, 3 * h, h, ACT_NONE, st));
         }
         DecodeAttnArgs da;
         da.qkv = m->qkv.p;
@@ -550,7 +606,11 @@ int decode_step_launch(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
         } else {
             B2_TRY(decode_attn_bf16(da, st));
         }
-        if (f8) {
+        if (small4) {
+            B2_TRY(gemv4(m->attn.p, h, L.q_o, L.a_o, nullptr, 0.f, m->x.p, h, m->x.p, h, B, h, h, ACT_NONE, st));
+            B2_TRY(gemv4(m->x.p, h, L.q_gu, L.a_gu, L.ln2.p, d.rms_eps, nullptr, 0, m->act.p, I, B, 2 * I, h, ACT_SWIGLU, st));
+            B2_TRY(gemv4(m->act.p, I, L.q_d, L.a_d, nullptr, 0.f, m->x.p, h, m->x.p, h, B, h, I, ACT_NONE, st));
+        } else if (f8) {
             B2_TRY(quantize_rows_e4m3(m->attn.p, h, B, h, m->xq8.p, h, m->xscale.as<float>(), st));
             B2_TRY(skinny8(m, kv, L.wo8.p, L.s_o.as<float>(), m->x.p, h, m->x.p, h, 0, B, h, h, ACT_NONE, st));
             B2_TRY(rmsnorm_quant_e4m3(m->x.p, h, L.ln2.p, m->xq8.p, h, m->xscale.as<float>(), B, h, d.rms_eps, st));
@@ -563,21 +623,21 @@ int decode_step_launch(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
                         ACT_SWIGLU, st));
             B2_TRY(gemv(m->act.p, I, L.wd.p, I, nullptr, 0.f, m->x.p, h, m->x.p, h, 0, B, h, I, ACT_NONE, st));
         } else if (sk) {
-            B2_TRY(skinny(kv, m->attn.p, h, L.wo.p, h, m->x.p, h, m->x.p, h, 0, B, h, h, ACT_NONE, st));
+            B2_TRY(skinny(kv, m->attn.p, h, lw.wo, h, m->x.p, h, m->x.p, h, 0, B, h, h, ACT_NONE, st));
             B2_TRY(rmsnorm_bf16(m->x.p, h, L.ln2.p, m->xn.p, B, h, d.rms_eps, st));
-            B2_TRY(skinny(kv, m->xn.p, h, L.wgu.p, h, nullptr, 0, m->act.p, I, 0, B, 2 * I, h, ACT_SWIGLU, st));
-            B2_TRY(skinny(kv, m->act.p, I, L.wd.p, I, m->x.p, h, m->x.p, h, 0, B, h, I, ACT_NONE, st));
+            B2_TRY(skinny(kv, m->xn.p, h, lw.wgu, h, nullptr, 0, m->act.p, I, 0, B, 2 * I, h, ACT_SWIGLU, st));
+            B2_TRY(skinny(kv, m->act.p, I, lw.wd, I, m->x.p, h, m->x.p, h, 0, B, h, I, ACT_NONE, st));
         } else {
-            B2_TRY(gemm(m->attn.p, h, L.wo.p, h, nullptr, m->x.p, h, m->x.p, h, 0, B, h, h, ACT_NONE, st));
+            B2_TRY(gemm(m->attn.p, h, lw.wo, h, nullptr, m->x.p, h, m->x.p, h, 0, B, h, h, ACT_NONE, st));
             B2_TRY(rmsnorm_bf16(m->x.p, h, L.ln2.p, m->xn.p, B, h, d.rms_eps, st));
-            B2_TRY(gemm(m->xn.p, h, L.wgu.p, h, nullptr, nullptr, 0, m->act.p, I, 0, B, 2 * I, h, ACT_SWIGLU, st));
-            B2_TRY(gemm(m->act.p, I, L.wd.p, I, nullptr, m->x.p, h, m->x.p, h, 0, B, h, I, ACT_NONE, st));
+            B2_TRY(gemm(m->xn.p, h, lw.wgu, h, nullptr, nullptr, 0, m->act.p, I, 0, B, 2 * I, h, ACT_SWIGLU, st));
+            B2_TRY(gemm(m->act.p, I, lw.wd, I, nullptr, m->x.p, h, m->x.p, h, 0, B, h, I, ACT_NONE, st));
         }
     }
     if (f8) {
         B2_TRY(rmsnorm_quant_e4m3(m->x.p, h, m->final_norm.p, m->xq8.p, h, m->xscale.as<float>(), B, h, d.rms_eps, st));
         B2_TRY(skinny8(m, kv, m->lm_head8.p, m->s_head.as<float>(), nullptr, 0, m->logits.p, V, 1, B, V, h, ACT_NONE, st));
-    } else if (small) {
+    } else if (small || (small4 && gemv_fits(B, V, h, ACT_NONE))) {
         B2_TRY(gemv(m->x.p, h, m->lm_head.p, h, m->final_norm.p, d.rms_eps, nullptr, 0, m->logits.p, V, 1, B, V, h,
                     ACT_NONE, st));
     } else if (sk) {
@@ -628,6 +688,7 @@ int join_stream(b2_kv* kv, cudaStream_t st, cudaStream_t run) {
 // run one step, through the cached CUDA graph when possible
 bool use_mega(const b2_model* m, const b2_kv* kv, int B) {
     if (kv->e4m3()) return false;  // the megakernel reads bf16 caches only: an e4m3 cache takes the multi-kernel step at every batch
+    if (m->nf4) return false;      // ... and bf16 weights only
     if (!decode_mega_fits(B, m->d.hidden, m->d.inter) || m->d.layers > 48) return false;
     static int flag = -1;
     if (flag < 0) {
@@ -738,6 +799,13 @@ int decode_step_run(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     }
     B2_CUDA_CHECK(cudaGraphLaunch(kv->graph, st));
     // kernels per step: embed + L*(qkv, attn, o, gate/up, down [+2 norms when B>8]) + head(+norm) + sample_publish
+    // (NF4: 5 per layer with gemv_nf4, otherwise the dequantisation of the layer in front of the 7)
+    if (m->nf4) {
+        const bool small4 = use_gemv_nf4(m, B);
+        const bool head_gemv = small4 && gemv_fits(B, m->d.vocab, m->d.hidden, ACT_NONE);
+        g_launch_count += 1 + (unsigned long long)m->d.layers * (small4 ? 5 : 8) + (head_gemv ? 1 : 2) + 1;
+        return 0;
+    }
     const bool small = !use_skinny(kv, B) && B <= 8 && gemv_fits(B, m->d.hidden, m->d.inter, ACT_NONE) &&
                        gemv_fits(B, m->d.vocab, m->d.hidden, ACT_NONE);
     const int per_layer = small ? 5 : ((m->fp8_decode && use_skinny(kv, B)) ? 9 : 7);
@@ -789,7 +857,7 @@ int b2_init(int device) {
 }
 
 const char* b2_last_error(void) { return g_err; }
-int b2_version(void) { return 4; }
+int b2_version(void) { return 5; }
 unsigned long long b2_launch_count(void) { return g_launch_count; }
 
 int b2_model_create(const b2_model_desc* desc, b2_model** out) {
@@ -844,6 +912,9 @@ int b2_model_set_weight(b2_model* m, const char* hf_key, const void* ptr, const 
     } else if (k == "lm_head.weight") {
         B2_TRY(expect_shape(hf_key, shape, ndim, V, h));
         r = put(m->lm_head, (size_t)V * h, 0, ptr, dtype, (int64_t)V * h);
+    } else if (m->nf4 && (k == "model.mm_projector.0.weight" || k == "model.mm_projector.2.weight")) {
+        set_error("set_weight(%s): the projector of this model holds its NF4 w_hat (b2_model_enable_nf4); it cannot be reloaded", hf_key);
+        return -1;
     } else if (k == "model.mm_projector.0.weight") {
         B2_TRY(expect_shape(hf_key, shape, ndim, h, D));
         r = put(m->p0_w, (size_t)h * D, 0, ptr, dtype, (int64_t)h * D);
@@ -966,15 +1037,16 @@ int b2_model_destroy(b2_model* m) {
                      &m->embed, &m->final_norm, &m->lm_head, &m->v_col, &m->v_patch, &m->v_hidden, &m->v_xn,
                      &m->v_qkv, &m->v_attn, &m->v_mlp, &m->v_feats, &m->p_mid, &m->p_done, &m->enc_pixels, &m->enc_out, &m->x, &m->xn, &m->qkv, &m->attn,
                      &m->act, &m->last_idx, &m->chunk_pos, &m->xlast, &m->logits, &m->splice_idx, &m->lm_head8, &m->s_head, &m->xq8, &m->xscale,
-                     &m->kstage, &m->vstage};
+                     &m->kstage, &m->vstage, &m->nf4_scratch};
     for (DevBuf* b : top) b->free();
     for (VitLayer& L : m->vit) {
         DevBuf* bs[12] = {&L.ln1_g, &L.ln1_b, &L.wqkv, &L.bqkv, &L.wo, &L.bo, &L.ln2_g, &L.ln2_b, &L.w1, &L.b1, &L.w2, &L.b2};
         for (DevBuf* b : bs) b->free();
     }
     for (LlamaLayer& L : m->ll) {
-        DevBuf* bs[16] = {&L.ln1, &L.wqkv, &L.wo, &L.ln2, &L.wgu, &L.wd, &L.tmp_gate, &L.tmp_up,
-                          &L.wqkv8, &L.wo8, &L.wgu8, &L.wd8, &L.s_qkv, &L.s_o, &L.s_gu, &L.s_d};
+        DevBuf* bs[24] = {&L.ln1, &L.wqkv, &L.wo, &L.ln2, &L.wgu, &L.wd, &L.tmp_gate, &L.tmp_up,
+                          &L.wqkv8, &L.wo8, &L.wgu8, &L.wd8, &L.s_qkv, &L.s_o, &L.s_gu, &L.s_d,
+                          &L.q_qkv, &L.a_qkv, &L.q_o, &L.a_o, &L.q_gu, &L.a_gu, &L.q_d, &L.a_d};
         for (DevBuf* b : bs) b->free();
     }
     delete m;
@@ -989,6 +1061,7 @@ int b2_model_enable_fp8_decode(b2_model* m) {
     std::lock_guard<std::mutex> lk(m->mu);
     DeviceGuard dg(m->device);
     if (m->fp8_decode) return 0;
+    B2_CHECK_ARG(!m->nf4, "b2_model_enable_fp8_decode: the decoder Linears are NF4 (b2_model_enable_nf4); the two formats do not combine");
     const b2_model_desc& d = m->d;
     const int h = d.hidden, I = d.inter, V = d.vocab;
     B2_CHECK_ARG(h % 16 == 0 && I % 16 == 0, "b2_model_enable_fp8_decode: hidden/inter must be multiples of 16");
@@ -1010,6 +1083,87 @@ int b2_model_enable_fp8_decode(b2_model* m) {
     B2_CUDA_CHECK(cudaDeviceSynchronize());
     m->fp8_decode = true;
     return 0;
+}
+
+// load_4bit (reference llava/model/builder.py:26-41): the seven decoder Linears of every layer become NF4 (codes in GEMV order
+// + fp32 absmax per 64-element block) and their bf16 buffers are freed; both projector weights are replaced by their w_hat in
+// place (the projector kernels stay bf16); the one-layer dequantisation scratch of prefill and batch > 8 decode is allocated.
+int b2_model_enable_nf4(b2_model* m) {
+    B2_CHECK_ARG(m != nullptr, "b2_model_enable_nf4: null model");
+    std::lock_guard<std::mutex> lk(m->mu);
+    DeviceGuard dg(m->device);
+    B2_CHECK_ARG(m->finalized, "b2_model_enable_nf4: model not finalized");
+    if (m->nf4) return 0;
+    B2_CHECK_ARG(!m->fp8_decode, "b2_model_enable_nf4: e4m3 decode weights are enabled (b2_model_enable_fp8_decode); the two formats do not combine");
+    B2_CHECK_ARG(m->kv_live.load() == 0, "b2_model_enable_nf4: %d KV cache(s) exist; enable NF4 before creating any (the megakernel "
+                 "tables of existing caches point at the bf16 weights)", m->kv_live.load());
+    const b2_model_desc& d = m->d;
+    const int h = d.hidden, I = d.inter, D = d.vit_hidden;
+    auto quant = [&](const DevBuf& w, int N, int K, DevBuf& q, DevBuf& a) -> int {
+        B2_TRY(q.alloc((size_t)N * K / 2));
+        B2_TRY(a.alloc((size_t)N * (K / 64) * sizeof(float)));
+        return quantize_nf4(w.p, K, N, K, q.p, a.as<float>(), 1, nullptr);
+    };
+    int r = 0;
+    for (LlamaLayer& L : m->ll) {
+        if ((r = quant(L.wqkv, 3 * h, h, L.q_qkv, L.a_qkv)) != 0 || (r = quant(L.wo, h, h, L.q_o, L.a_o)) != 0 ||
+            (r = quant(L.wgu, 2 * I, h, L.q_gu, L.a_gu)) != 0 || (r = quant(L.wd, h, I, L.q_d, L.a_d)) != 0)
+            break;
+    }
+    // projector: w -> codes (canonical) -> w_hat, in place
+    DevBuf pq, pa;
+    // w -> codes (canonical) -> w_hat into a new buffer; the projector's own buffers are swapped in only when both succeeded
+    auto roundtrip = [&](const DevBuf& w, int N, int K, DevBuf& out) -> int {
+        B2_TRY(pq.alloc((size_t)N * K / 2));
+        B2_TRY(pa.alloc((size_t)N * (K / 64) * sizeof(float)));
+        B2_TRY(out.alloc((size_t)N * K * 2));
+        B2_TRY(quantize_nf4(w.p, K, N, K, pq.p, pa.as<float>(), 0, nullptr));
+        Nf4Matrix mt;
+        mt.q = pq.p; mt.absmax = pa.as<float>(); mt.out = out.p; mt.N = N; mt.K = K;
+        B2_TRY(dequantize_nf4(&mt, 1, 0, nullptr));
+        B2_CUDA_CHECK(cudaStreamSynchronize(nullptr));
+        return 0;
+    };
+    DevBuf p0_hat, p2_hat;
+    if (r == 0) r = m->nf4_scratch.alloc(((size_t)4 * h * h + (size_t)3 * I * h) * 2);
+    if (r == 0 && cudaDeviceSynchronize() != cudaSuccess) { set_error("b2_model_enable_nf4: quantisation failed: %s", cudaGetErrorString(cudaGetLastError())); r = -2; }
+    if (r == 0) r = roundtrip(m->p0_w, h, D, p0_hat);
+    if (r == 0) r = roundtrip(m->p2_w, h, h, p2_hat);
+    pq.free();
+    pa.free();
+    if (r != 0) {  // nothing of the model has changed yet
+        for (LlamaLayer& L : m->ll)
+            for (DevBuf* b : {&L.q_qkv, &L.a_qkv, &L.q_o, &L.a_o, &L.q_gu, &L.a_gu, &L.q_d, &L.a_d}) b->free();
+        m->nf4_scratch.free();
+        p0_hat.free();
+        p2_hat.free();
+        return r;
+    }
+    std::swap(m->p0_w, p0_hat);
+    std::swap(m->p2_w, p2_hat);
+    p0_hat.free();  // now the bf16 originals
+    p2_hat.free();
+    for (LlamaLayer& L : m->ll)
+        for (DevBuf* b : {&L.wqkv, &L.wo, &L.wgu, &L.wd}) b->free();
+    m->nf4 = true;
+    return 0;
+}
+
+int64_t b2_model_weight_bytes(b2_model* m) {
+    B2_CHECK_ARG(m != nullptr, "b2_model_weight_bytes: null model");
+    std::lock_guard<std::mutex> lk(m->mu);
+    size_t n = 0;
+    for (const DevBuf* b : {&m->patch_w, &m->cls, &m->pos, &m->pre_g, &m->pre_b, &m->p0_w, &m->p0_b, &m->p2_w, &m->p2_b, &m->embed,
+                            &m->final_norm, &m->lm_head, &m->lm_head8, &m->s_head})
+        n += b->bytes;
+    for (const VitLayer& L : m->vit)
+        for (const DevBuf* b : {&L.ln1_g, &L.ln1_b, &L.wqkv, &L.bqkv, &L.wo, &L.bo, &L.ln2_g, &L.ln2_b, &L.w1, &L.b1, &L.w2, &L.b2})
+            n += b->bytes;
+    for (const LlamaLayer& L : m->ll)
+        for (const DevBuf* b : {&L.ln1, &L.wqkv, &L.wo, &L.ln2, &L.wgu, &L.wd, &L.wqkv8, &L.wo8, &L.wgu8, &L.wd8, &L.s_qkv, &L.s_o,
+                                &L.s_gu, &L.s_d, &L.q_qkv, &L.a_qkv, &L.q_o, &L.a_o, &L.q_gu, &L.a_gu, &L.q_d, &L.a_d})
+            n += b->bytes;
+    return (int64_t)n;
 }
 
 int b2_kv_create(b2_model* m, int max_batch, int max_seq, b2_kv** out) {
@@ -1051,7 +1205,7 @@ int b2_kv_create_ex(b2_model* m, int max_batch, int max_seq, int kv_dtype, b2_kv
     }
     kv->out_capacity = max_seq;
     const int max_split = 64;
-    {
+    if (!m->nf4) {  // the megakernel reads bf16 weights; an NF4 model never takes it (use_mega)
         std::vector<MegaLayer> tbl(m->d.layers);
         for (int l = 0; l < m->d.layers; ++l) {
             LlamaLayer& L = m->ll[l];
@@ -1122,6 +1276,8 @@ int b2_kv_create_ex(b2_model* m, int max_batch, int max_seq, int kv_dtype, b2_kv
     // (seen in scripts/decode_ab.py FRESHKV=1: different tokens on a cache that was created a moment earlier).
     B2_CUDA_CHECK(cudaDeviceSynchronize());
     kv->len_host.assign(max_batch, 0);
+    kv->counted = true;
+    m->kv_live++;
     *out = kv;
     return 0;
 }
@@ -1148,6 +1304,7 @@ int b2_kv_destroy(b2_kv* kv) {
     if (kv == nullptr) return 0;
     DeviceGuard dg(kv->m->device);
     cudaDeviceSynchronize();
+    if (kv->counted) kv->m->kv_live--;
     if (kv->ring_host) cudaFreeHost(kv->ring_host);
     if (kv->graph) cudaGraphExecDestroy(kv->graph);
     if (kv->own_stream) cudaStreamDestroy(kv->own_stream);
@@ -1333,6 +1490,8 @@ int b2_prefill_at(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* sta
     { const char* e = getenv("B2_ROPE_FUSED"); if (e != nullptr && e[0] == '0') rope_fused = false; }
     for (int l = 0; l < d.layers; ++l) {
         LlamaLayer& L = m->ll[l];
+        LayerW lw;
+        B2_TRY(layer_weights(m, l, &lw, st));
         bf16* kc = q8 ? m->kstage.as<bf16>() : reinterpret_cast<bf16*>(kv->k_layer(l)) + slot_rows * m->hd;
         bf16* vc = q8 ? m->vstage.as<bf16>() : reinterpret_cast<bf16*>(kv->v_layer(l)) + slot_rows * m->hd;
         const size_t row0 = (size_t)l * kv->layer_rows() + slot_rows;  // e4m3: first scale / row of this layer's slots
@@ -1344,13 +1503,13 @@ int b2_prefill_at(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* sta
         if (rope_fused) {
             // QKV projection with RoPE and the cache write in its epilogue (CTA-pair kernel): q -> qkv buffer, k / v -> cache
             GemmArgs g;
-            g.A = m->xn.p; g.lda = h; g.W = L.wqkv.p; g.ldw = h; g.out = m->qkv.p; g.ld_out = 3 * h;
+            g.A = m->xn.p; g.lda = h; g.W = lw.wqkv; g.ldw = h; g.out = m->qkv.p; g.ld_out = 3 * h;
             g.M = T; g.N = 3 * h; g.K = h; g.act = ACT_ROPE_QKV;
             g.rope.table = kv->rope_tab.p; g.rope.kcache = kc; g.rope.vcache = vc; g.rope.S = S; g.rope.H = H; g.rope.Smax = kv_pitch;
             g.rope.pos0 = offset ? pos_dev : nullptr;
             B2_TRY(gemm_bf16_2cta(g, st));
         } else {
-            B2_TRY(gemm(m->xn.p, h, L.wqkv.p, h, nullptr, nullptr, 0, m->qkv.p, 3 * h, 0, T, 3 * h, h, ACT_NONE, st));
+            B2_TRY(gemm(m->xn.p, h, lw.wqkv, h, nullptr, nullptr, 0, m->qkv.p, 3 * h, 0, T, 3 * h, h, ACT_NONE, st));
             B2_TRY(rope_kv_write(m->qkv.p, kc, vc, B, S, H, m->hd, kv_pitch, d.rope_theta, st, offset ? pos_dev : nullptr));
         }
         FlashArgs fa;
@@ -1369,10 +1528,10 @@ int b2_prefill_at(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* sta
                                     offset ? clen_dev : kv->len_dev.as<int32_t>() + slot0, B, S, H, m->hd, kv->pitch, st,
                                     offset ? pos_dev : nullptr, kv_pitch));
         }
-        B2_TRY(gemm(m->attn.p, h, L.wo.p, h, nullptr, m->x.p, h, m->x.p, h, 0, T, h, h, ACT_NONE, st));
+        B2_TRY(gemm(m->attn.p, h, lw.wo, h, nullptr, m->x.p, h, m->x.p, h, 0, T, h, h, ACT_NONE, st));
         B2_TRY(rmsnorm_bf16(m->x.p, h, L.ln2.p, m->xn.p, T, h, d.rms_eps, st));
-        B2_TRY(gemm(m->xn.p, h, L.wgu.p, h, nullptr, nullptr, 0, m->act.p, I, 0, T, 2 * I, h, ACT_SWIGLU, st));
-        B2_TRY(gemm(m->act.p, I, L.wd.p, I, nullptr, m->x.p, h, m->x.p, h, 0, T, h, I, ACT_NONE, st));
+        B2_TRY(gemm(m->xn.p, h, lw.wgu, h, nullptr, nullptr, 0, m->act.p, I, 0, T, 2 * I, h, ACT_SWIGLU, st));
+        B2_TRY(gemm(m->act.p, I, lw.wd, I, nullptr, m->x.p, h, m->x.p, h, 0, T, h, I, ACT_NONE, st));
     }
     if (logits_mode == B2_LOGITS_LAST) {
         // only the last valid position per sample feeds generation (the reference computes lm_head on all S)
@@ -1777,6 +1936,25 @@ int b2_op_gemv(const void* x, int64_t ldx, const void* W, int ldw, const void* n
     B2_CHECK_ARG(x && W && out, "b2_op_gemv: null argument");
     return gemv(x, ldx, W, ldw, norm_gamma, eps, residual, ld_res, out, ld_out, out_fp32, B, N, K, act,
                 reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2_op_quantize_nf4(const void* w, int N, int K, void* codes, float* absmax, void* stream) {
+    return quantize_nf4(w, K, N, K, codes, absmax, 0, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2_op_dequantize_nf4(const void* codes, const float* absmax, int N, int K, void* out, void* stream) {
+    Nf4Matrix mt;
+    mt.q = codes; mt.absmax = absmax; mt.out = out; mt.N = N; mt.K = K;
+    return dequantize_nf4(&mt, 1, 0, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2_op_gemv_nf4(const void* x, int64_t ldx, const void* codes, const float* absmax, const void* norm_gamma, float eps,
+                   const void* residual, int ld_res, void* out, int ld_out, int B, int N, int K, int act, void* stream) {
+    B2_CHECK_ARG(x && codes && absmax && out, "b2_op_gemv_nf4: null argument");
+    GemvArgs g;
+    g.x = x; g.ldx = ldx; g.norm_gamma = norm_gamma; g.eps = eps; g.residual = residual; g.ld_res = ld_res;
+    g.out = out; g.ld_out = ld_out; g.B = B; g.N = N; g.K = K; g.act = act;
+    return gemv_nf4(g, codes, absmax, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int b2_op_gemm_skinny(const void* x, int ldx, const void* W, int ldw, const void* residual, int ld_res, void* out,

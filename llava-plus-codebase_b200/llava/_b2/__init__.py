@@ -78,6 +78,8 @@ SIGNATURES = {
     "b2_model_finalize": (_i32, [_vp]),
     "b2_model_destroy": (_i32, [_vp]),
     "b2_model_enable_fp8_decode": (_i32, [_vp]),
+    "b2_model_enable_nf4": (_i32, [_vp]),
+    "b2_model_weight_bytes": (_i64, [_vp]),
     "b2_kv_create": (_i32, [_vp, _i32, _i32, _c.POINTER(_vp)]),
     "b2_kv_create_ex": (_i32, [_vp, _i32, _i32, _i32, _c.POINTER(_vp)]),
     "b2_kv_dtype": (_i32, [_vp]),
@@ -109,6 +111,9 @@ SIGNATURES = {
     "b2_beam_step": (_i32, [_vp, _vp, _c.POINTER(BeamStepArgs), _vp]),
     "b2_op_gemm": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "b2_op_gemv": (_i32, [_vp, _i64, _vp, _i32, _vp, _f32, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
+    "b2_op_quantize_nf4": (_i32, [_vp, _i32, _i32, _vp, _vp, _vp]),
+    "b2_op_dequantize_nf4": (_i32, [_vp, _vp, _i32, _i32, _vp, _vp]),
+    "b2_op_gemv_nf4": (_i32, [_vp, _i64, _vp, _vp, _vp, _f32, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
     "b2_op_gemm_skinny": (_i32, [_vp, _i32, _vp, _i32, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _vp]),
     "b2_op_gemm_skinny_fp8": (_i32, [_vp, _i32, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _vp]),
     "b2_op_quantize_rows_e4m3": (_i32, [_vp, _i64, _i32, _i32, _vp, _i64, _vp, _vp]),
@@ -286,6 +291,16 @@ class Engine:
         """BASELINE configs[4]: e4m3 weights for decode at batch >= 7 (see include/b2llava.h): W8A8 numerics, opt-in."""
         with torch.cuda.device(self.index):
             check(self.lib.b2_model_enable_fp8_decode(self.handle), "b2_model_enable_fp8_decode")
+
+    def enable_nf4(self):
+        """load_4bit: NF4 decoder Linears and a w_hat projector (see include/b2llava.h). Call after finalize() and before any
+        KV cache exists; it cannot be combined with enable_fp8_decode()."""
+        with torch.cuda.device(self.index):
+            check(self.lib.b2_model_enable_nf4(self.handle), "b2_model_enable_nf4")
+
+    def weight_bytes(self):
+        """Device bytes of the weights the engine holds (workspaces excluded)."""
+        return int(self.lib.b2_model_weight_bytes(self.handle))
 
     def new_kv(self, max_batch, max_seq, dtype="bf16"):
         with torch.cuda.device(self.index):

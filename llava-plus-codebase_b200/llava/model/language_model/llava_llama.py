@@ -298,6 +298,7 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         # cache bytes, decode numerics change — include/b2llava.h, b2_kv_create_ex); checked before anything is allocated
         self._kv_dtype = getattr(c, "b2_kv_dtype", None) or os.environ.get("B2_KV_DTYPE") or "bf16"
         kv_dtype_code(self._kv_dtype)
+        weight_format = _check_weight_format(c)
         max_seq = self._limits["max_seq"] or min(getattr(c, "max_position_embeddings", 4096), 4096)
         desc = dict(
             image_size=vc.image_size, patch_size=vc.patch_size, vit_hidden=vc.hidden_size,
@@ -318,6 +319,8 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 continue
             eng.set_weight(k, v.to(self.device))
         eng.finalize()
+        if weight_format == "nf4":  # load_4bit: before any KV cache exists
+            eng.enable_nf4()
         # BASELINE configs[4] opt-in: e4m3 decoder weights for batch >= 7 decode (config.b2_fp8_decode or B2_FP8_DECODE=1)
         if getattr(c, "b2_fp8_decode", False) or os.environ.get("B2_FP8_DECODE") == "1":
             eng.enable_fp8_decode()
@@ -795,15 +798,20 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
     def from_pretrained(cls, pretrained_model_name_or_path, *model_args, config=None, torch_dtype=None,
                         low_cpu_mem_usage=True, device_map=None, device=None, **kwargs):
         """Minimal HF-style loader: `config.json` + safetensors / pytorch_model*.bin shards in a local directory
-        (ref builder.py:105-106 calls this). 8-bit/4-bit bitsandbytes loading is not part of the H100 path."""
-        if kwargs.get("load_in_8bit") or kwargs.get("load_in_4bit") or kwargs.get("quantization_config") is not None:
-            raise NotImplementedError("bitsandbytes quantised loading is not supported on the H100 path")
+        (ref builder.py:105-106 calls this). 4-bit loading (`load_in_4bit=True`, or a `quantization_config` — a
+        transformers BitsAndBytesConfig or a dict — with load_in_4bit and bnb_4bit_quant_type "nf4") sets
+        config.b2_weight_format = "nf4": the engine then holds NF4 decoder Linears (include/b2llava.h,
+        b2_model_enable_nf4). 8-bit loading and FP4 are not part of the H100 path."""
+        nf4 = _nf4_requested(kwargs)
         path = pretrained_model_name_or_path
         if not os.path.isdir(path):
             raise ValueError(f"{path!r} is not a local checkpoint directory (no network access on this path)")
         if config is None:
             with open(os.path.join(path, "config.json")) as f:
                 config = LlavaConfig(**json.load(f))
+        if nf4:
+            config.b2_weight_format = "nf4"
+            _check_weight_format(config)
         dev = device
         if dev is None and isinstance(device_map, (str, torch.device)) and str(device_map) not in ("auto",):
             dev = device_map
@@ -823,6 +831,35 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
 
     def eval(self):
         return super().eval()
+
+
+def _nf4_requested(kwargs):
+    """True when from_pretrained's arguments ask for bitsandbytes NF4 (the reference's load_4bit); raises NotImplementedError
+    for the quantised loads this package does not serve (8-bit, FP4)."""
+    qc = kwargs.get("quantization_config")
+    if kwargs.get("load_in_8bit"):
+        raise NotImplementedError("8-bit (LLM.int8) loading is not part of the H100 path")
+    if qc is None:
+        return bool(kwargs.get("load_in_4bit"))
+    get = qc.get if isinstance(qc, dict) else (lambda k, d=None: getattr(qc, k, d))
+    if get("load_in_8bit", False):
+        raise NotImplementedError("8-bit (LLM.int8) loading is not part of the H100 path")
+    if not get("load_in_4bit", False):
+        raise NotImplementedError("quantization_config without load_in_4bit: only bitsandbytes NF4 is served")
+    qt = get("bnb_4bit_quant_type", "fp4")  # BitsAndBytesConfig's own default
+    if qt != "nf4":
+        raise NotImplementedError(f"bnb_4bit_quant_type={qt!r}: only 'nf4' is served")
+    return True
+
+
+def _check_weight_format(config):
+    """config.b2_weight_format: None / "bf16" (default) or "nf4"; NF4 and the e4m3 decode weights do not combine."""
+    fmt = getattr(config, "b2_weight_format", None) or "bf16"
+    if fmt not in ("bf16", "nf4"):
+        raise ValueError(f"unknown b2_weight_format {fmt!r}: expected 'bf16' or 'nf4'")
+    if fmt == "nf4" and (getattr(config, "b2_fp8_decode", False) or os.environ.get("B2_FP8_DECODE") == "1"):
+        raise ValueError("b2_weight_format='nf4' (load_4bit) cannot be combined with b2_fp8_decode (e4m3 decode weights)")
+    return fmt
 
 
 def _stream_decode(engine, kv, logits, sampling, B, max_new_tokens, eos_ids, pad, prompt, streamer, stopping_criteria,
