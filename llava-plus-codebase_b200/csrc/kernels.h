@@ -292,10 +292,8 @@ int argmax_f32(const float* logits, int B, int V, int32_t* out, cudaStream_t str
 struct I32Pack { int32_t v[128]; };
 // dst_a[i] = a_host[i] (and dst_b[i] = b_host[i] when dst_b != null), i < n: values travel as kernel parameters
 int set_i32_pairs(int32_t* dst_a, const int32_t* a_host, int32_t* dst_b, const int32_t* b_host, int n, cudaStream_t stream);
-int add_i32(int32_t* x, int n, int delta, cudaStream_t stream);
 int convert_to_bf16(const void* src, int src_dtype, void* dst, int64_t n, cudaStream_t stream);
 // out[2I, h]: within each 128-row group g: rows [0,64) = gate[g*64 .. +64), rows [64,128) = up[g*64 .. +64)
 int interleave_gate_up(const void* gate, const void* up, void* out, int I, int h, cudaStream_t stream);
-int store_token(const int32_t* src, int32_t* dst_base, const int32_t* step_counter, int B, cudaStream_t stream);
 
 }  // namespace b2

@@ -94,11 +94,6 @@ __global__ void __launch_bounds__(1024) argmax_kernel(const float* __restrict__ 
     }
 }
 
-__global__ void add_i32_kernel(int32_t* x, int n, int delta) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) x[i] += delta;
-}
-
 template <typename T>
 __device__ __forceinline__ float to_f32(T v);
 template <>
@@ -121,13 +116,6 @@ __global__ void interleave_gate_up_kernel(const uint4* __restrict__ gate, const 
                                 : up + (size_t)(grp * 64 + r - 64) * vec_per_row;
     uint4* o = out + (size_t)orow * vec_per_row;
     for (int c = threadIdx.x; c < vec_per_row; c += blockDim.x) o[c] = src[c];
-}
-
-// dst[step*B + b] = src[b]; step read from device memory so the launch can be replayed from a CUDA graph
-__global__ void store_token_kernel(const int32_t* __restrict__ src, int32_t* __restrict__ dst_base,
-                                   const int32_t* __restrict__ step_counter, int B) {
-    const int b = threadIdx.x;
-    if (b < B) dst_base[(size_t)(*step_counter) * B + b] = src[b];
 }
 
 // Device half of the splice INDEX (llava/model/llava_arch.py:143-187 of the reference, equal-length unpadded rows): one CTA
@@ -241,12 +229,6 @@ int argmax_f32(const float* logits, int B, int V, int32_t* out, cudaStream_t str
     return 0;
 }
 
-int add_i32(int32_t* x, int n, int delta, cudaStream_t stream) {
-    add_i32_kernel<<<(n + 127) / 128, 128, 0, stream>>>(x, n, delta);
-    B2_LAUNCH_CHECK();
-    return 0;
-}
-
 int convert_to_bf16(const void* src, int src_dtype, void* dst, int64_t n, cudaStream_t stream) {
     if (n == 0) return 0;
     if (src_dtype == DT_BF16) {
@@ -273,13 +255,6 @@ int interleave_gate_up(const void* gate, const void* up, void* out, int I, int h
     interleave_gate_up_kernel<<<2 * I, 128, 0, stream>>>(reinterpret_cast<const uint4*>(gate),
                                                          reinterpret_cast<const uint4*>(up),
                                                          reinterpret_cast<uint4*>(out), I, h / 8);
-    B2_LAUNCH_CHECK();
-    return 0;
-}
-
-int store_token(const int32_t* src, int32_t* dst_base, const int32_t* step_counter, int B, cudaStream_t stream) {
-    B2_CHECK_ARG(B <= 1024, "store_token: B too large");
-    store_token_kernel<<<1, B < 32 ? 32 : ((B + 31) / 32) * 32, 0, stream>>>(src, dst_base, step_counter, B);
     B2_LAUNCH_CHECK();
     return 0;
 }

@@ -9,6 +9,7 @@
 #include <string.h>
 #include <time.h>
 
+#include <array>
 #include <atomic>
 #include <utility>
 #include <mutex>
@@ -67,16 +68,30 @@ struct VitLayer {
     DevBuf ln1_g, ln1_b, wqkv, bqkv, wo, bo, ln2_g, ln2_b, w1, b1, w2, b2;
     unsigned qkv_w = 0, qkv_b = 0;  // bit j set: part j (q/k/v) of the fused buffer has arrived
 };
+// One decoder Linear [N, K] in each format it can be held in: the bf16 weight w, its e4m3 copy w8 + per-row fp32 scales s8
+// (b2_model_enable_fp8_decode), and its NF4 codes q in GEMV order [N, K/2] + absmax a [N, K/64] (b2_model_enable_nf4, which
+// frees w)
+struct Linear {
+    DevBuf w;
+    DevBuf w8, s8;
+    DevBuf q, a;
+    void free() { for (DevBuf* b : {&w, &w8, &s8, &q, &a}) b->free(); }
+    size_t bytes() const { return w.bytes + w8.bytes + s8.bytes + q.bytes + a.bytes; }
+};
 struct LlamaLayer {
-    DevBuf ln1, wqkv, wo, ln2, wgu, wd;
+    DevBuf ln1, ln2;
+    Linear qkv, o, gu, d;  // gu: gate / up rows interleaved in blocks of 64 (interleave_gate_up)
+    std::array<Linear*, 4> linears() { return {&qkv, &o, &gu, &d}; }  // the order of layer_shapes
     unsigned qkv_parts = 0;
-    DevBuf wqkv8, wo8, wgu8, wd8, s_qkv, s_o, s_gu, s_d;  // e4m3 copies + per-row fp32 scales (b2_model_enable_fp8_decode)
     DevBuf tmp_gate, tmp_up;  // staging until both halves arrived
-    // NF4 (b2_model_enable_nf4): codes in GEMV order [N, K/2] and absmax [N, K/64] of wqkv / wo / wgu / wd; the bf16 buffers
-    // above are freed
-    DevBuf q_qkv, a_qkv, q_o, a_o, q_gu, a_gu, q_d, a_d;
     bool has_gate = false, has_up = false;
 };
+struct LinearShape { int N, K, act; };
+// N, K and activation of a decoder layer's Linears: QKV, O, gate/up (SwiGLU), down
+std::array<LinearShape, 4> layer_shapes(const b2_model_desc& d) {
+    const int h = d.hidden, I = d.inter;
+    return {{{3 * h, h, ACT_NONE}, {h, h, ACT_NONE}, {2 * I, h, ACT_SWIGLU}, {h, I, ACT_NONE}}};
+}
 }  // namespace
 }  // namespace b2
 
@@ -93,7 +108,8 @@ struct b2_model {
     DevBuf patch_w, cls, pos, pre_g, pre_b;
     std::vector<VitLayer> vit;
     DevBuf p0_w, p0_b, p2_w, p2_b;
-    DevBuf embed, final_norm, lm_head;
+    DevBuf embed, final_norm;
+    Linear head;  // lm_head: w, and w8 / s8 with fp8 decode (never NF4)
     std::vector<LlamaLayer> ll;
     // errors detected by kernels (bad token ids / image rows): int[8] in mapped pinned host memory, slot = log2(B2_ERR_*)
     int* err_host = nullptr;
@@ -116,9 +132,9 @@ struct b2_model {
     cudaStream_t enc_stream = nullptr;       // capture is illegal on the legacy default stream: such callers run here
     cudaEvent_t enc_fork = nullptr, enc_join = nullptr;
     int enc_launches = 0;                    // kernels in one captured chunk (b2_launch_count bookkeeping)
-    // fp8 decode (BASELINE configs[4]): e4m3 lm_head + scales, quantised activation row buffer + per-token scales
+    // fp8 decode (BASELINE configs[4]): quantised activation row buffer + per-token scales
     bool fp8_decode = false;
-    DevBuf lm_head8, s_head, xq8, xscale;
+    DevBuf xq8, xscale;
     // e4m3 KV caches: one layer of roped bf16 K / V, [B][H][S][128], that prefill attends over before it is quantised into
     // the cache (allocated with the first e4m3 cache)
     DevBuf kstage, vstage;
@@ -143,6 +159,7 @@ struct b2_kv {
     // cached decode-step graph
     cudaGraphExec_t graph = nullptr;
     int graph_B = 0;
+    int graph_launches = 0;  // kernels in the captured step (b2_launch_count bookkeeping)
     // stream capture is illegal on the legacy default stream (torch's default current stream): decode steps
     // run on this library-owned stream, ordered against the caller's stream with events
     unsigned int mega_bar_base = 0;  // value of the grid-barrier counter before the next megakernel launch
@@ -249,34 +266,11 @@ int gemv(const void* x, int64_t ldx, const void* W, int ldw, const void* gamma, 
     return gemv_bf16(g, st);
 }
 
-// decode Linear at batch 9..128: swap-AB stream-K wgmma GEMM over the kv-owned workspace
-int skinny(b2_kv* kv, const void* x, int ldx, const void* W, int ldw, const void* res, int ld_res, void* out, int ld_out,
-           int out_fp32, int B, int N, int K, int act, cudaStream_t st) {
-    SkinnyArgs g;
-    g.x = x; g.ldx = ldx; g.W = W; g.ldw = ldw; g.residual = res; g.ld_res = ld_res;
-    g.out = out; g.ld_out = ld_out; g.out_fp32 = out_fp32; g.B = B; g.N = N; g.K = K; g.act = act;
-    g.partial = kv->sk_partial.as<float>(); g.partial_bytes = kv->sk_partial.bytes;
-    g.counters = kv->sk_counters.as<int>();
-    return gemm_skinny_bf16(g, st);
-}
 // Batch 7..128: below that the GEMV path (5 kernels/layer, RMSNorm fused) has fewer launches per layer than the stream-K GEMM
 // path (7 kernels/layer) and wins. B2_DECODE_SKINNY=0 selects the other paths for A/B runs (GEMV kernels for B <= 8, tile GEMM
-// with the batch padded to M=128 above), B2_DECODE_SKINNY=3 lowers the threshold to 3.
-// fp8 variant: xq8 / xscale hold the quantised activations of this GEMM
-int skinny8(b2_model* m, b2_kv* kv, const void* W8, const float* w_scale, const void* res, int ld_res, void* out, int ld_out,
-            int out_fp32, int B, int N, int K, int act, cudaStream_t st) {
-    SkinnyArgs g;
-    g.x = m->xq8.p; g.ldx = K; g.W = W8; g.ldw = K; g.residual = res; g.ld_res = ld_res;
-    g.out = out; g.ld_out = ld_out; g.out_fp32 = out_fp32; g.B = B; g.N = N; g.K = K; g.act = act;
-    g.partial = kv->sk_partial.as<float>(); g.partial_bytes = kv->sk_partial.bytes;
-    g.counters = kv->sk_counters.as<int>();
-    g.w_scale = w_scale; g.x_scale = m->xscale.as<float>();
-    return gemm_skinny_fp8(g, st);
-}
+// with the batch padded to M=128 above).
 bool use_skinny(const b2_kv* kv, int B) {
-    const char* e0 = getenv("B2_DECODE_SKINNY");
-    const int lo = (e0 != nullptr && e0[0] == '3') ? 3 : 7;
-    if (B < lo || B > 128 || kv->sk_partial.p == nullptr) return false;
+    if (B < 7 || B > 128 || kv->sk_partial.p == nullptr) return false;
     const char* e = getenv("B2_DECODE_SKINNY");
     return !(e != nullptr && e[0] == '0');
 }
@@ -286,17 +280,14 @@ bool use_skinny(const b2_kv* kv, int B) {
 struct LayerW { const void *wqkv, *wo, *wgu, *wd; };
 int layer_weights(b2_model* m, int l, LayerW* w, cudaStream_t st) {
     LlamaLayer& L = m->ll[l];
-    if (!m->nf4) { *w = {L.wqkv.p, L.wo.p, L.wgu.p, L.wd.p}; return 0; }
-    const int h = m->d.hidden, I = m->d.inter;
-    bf16* s = m->nf4_scratch.as<bf16>();
+    if (!m->nf4) { *w = {L.qkv.w.p, L.o.w.p, L.gu.w.p, L.d.w.p}; return 0; }
+    const auto lin = L.linears();
+    const auto sh = layer_shapes(m->d);
     Nf4Matrix mt[4];
-    const DevBuf* q[4] = {&L.q_qkv, &L.q_o, &L.q_gu, &L.q_d};
-    const DevBuf* a[4] = {&L.a_qkv, &L.a_o, &L.a_gu, &L.a_d};
-    const int N[4] = {3 * h, h, 2 * I, h}, K[4] = {h, h, h, I};
-    bf16* out = s;
+    bf16* out = m->nf4_scratch.as<bf16>();
     for (int i = 0; i < 4; ++i) {
-        mt[i].q = q[i]->p; mt[i].absmax = a[i]->as<float>(); mt[i].out = out; mt[i].N = N[i]; mt[i].K = K[i];
-        out += (size_t)N[i] * K[i];
+        mt[i].q = lin[i]->q.p; mt[i].absmax = lin[i]->a.as<float>(); mt[i].out = out; mt[i].N = sh[i].N; mt[i].K = sh[i].K;
+        out += (size_t)sh[i].N * sh[i].K;
     }
     B2_TRY(dequantize_nf4(mt, 4, 1, st));
     *w = {mt[0].out, mt[1].out, mt[2].out, mt[3].out};
@@ -304,16 +295,67 @@ int layer_weights(b2_model* m, int l, LayerW* w, cudaStream_t st) {
 }
 // NF4 decode at batch <= 8: gemv_nf4 for the seven decoder Linears when every shape fits its shared-memory budget
 bool use_gemv_nf4(const b2_model* m, int B) {
-    const int h = m->d.hidden, I = m->d.inter;
-    return m->nf4 && B <= 8 && gemv_nf4_fits(B, 3 * h, h, ACT_NONE) && gemv_nf4_fits(B, h, h, ACT_NONE) &&
-           gemv_nf4_fits(B, 2 * I, h, ACT_SWIGLU) && gemv_nf4_fits(B, h, I, ACT_NONE);
+    if (!m->nf4 || B > 8) return false;
+    for (const LinearShape& s : layer_shapes(m->d))
+        if (!gemv_nf4_fits(B, s.N, s.K, s.act)) return false;
+    return true;
 }
-int gemv4(const void* x, int64_t ldx, const DevBuf& q, const DevBuf& a, const void* gamma, float eps, const void* res, int ld_res,
-          void* out, int ld_out, int B, int N, int K, int act, cudaStream_t st) {
-    GemvArgs g;
-    g.x = x; g.ldx = ldx; g.norm_gamma = gamma; g.eps = eps; g.residual = res; g.ld_res = ld_res;
-    g.out = out; g.ld_out = ld_out; g.B = B; g.N = N; g.K = K; g.act = act;
-    return gemv_nf4(g, q.p, a.as<float>(), st);
+
+enum DecodePath { GEMV_NF4, SKINNY_FP8, GEMV, SKINNY, TILE };
+struct DecodePlan { DecodePath layer, head; };
+// Paths of the Linears of one multi-kernel decode step at batch B; the first row whose condition holds applies:
+//   condition                                     layer Linears   head
+//   use_gemv_nf4(m, B)                            GEMV_NF4        GEMV if gemv_fits(B, V, h), else TILE
+//   use_skinny(kv, B) && fp8 decode               SKINNY_FP8      SKINNY_FP8
+//   use_skinny(kv, B)                             SKINNY          SKINNY
+//   not NF4, B <= 8, gemv_fits every shape        GEMV            GEMV
+//   otherwise                                     TILE            TILE
+// GEMV: tensor-core GEMV kernels. SKINNY: swap-AB stream-K GEMM over the kv-owned workspace (weights streamed once, all SMs
+// busy); SKINNY_FP8 is the same GEMM on e4m3 weights x e4m3 activations. TILE: the wgmma tile GEMM. On an NF4 model SKINNY
+// and TILE read the layer layer_weights dequantised.
+DecodePlan decode_plan(const b2_model* m, const b2_kv* kv, int B) {
+    if (use_gemv_nf4(m, B)) return {GEMV_NF4, gemv_fits(B, m->d.vocab, m->d.hidden, ACT_NONE) ? GEMV : TILE};
+    if (use_skinny(kv, B)) return m->fp8_decode ? DecodePlan{SKINNY_FP8, SKINNY_FP8} : DecodePlan{SKINNY, SKINNY};
+    bool small = !m->nf4 && B <= 8 && gemv_fits(B, m->d.vocab, m->d.hidden, ACT_NONE);
+    for (const LinearShape& s : layer_shapes(m->d)) small = small && gemv_fits(B, s.N, s.K, s.act);
+    return small ? DecodePlan{GEMV, GEMV} : DecodePlan{TILE, TILE};
+}
+
+// One Linear of the multi-kernel decode step on `path`: out[B, N] = (rmsnorm(x; gamma) or x)[B, K] · W^T, plus out itself
+// when `residual` (x += ...). w_bf16 is the bf16 weight the GEMV / SKINNY / TILE paths read. GEMV and GEMV_NF4 fuse the norm;
+// SKINNY and TILE normalise into xn first; SKINNY_FP8 normalises (or only quantises) into xq8 / xscale.
+int decode_linear(b2_model* m, b2_kv* kv, DecodePath path, const Linear& lin, const void* w_bf16, const void* x, int ldx,
+                  const void* gamma, bool residual, void* out, int ld_out, int out_fp32, int B, int N, int K, int act,
+                  cudaStream_t st) {
+    const float eps = gamma ? m->d.rms_eps : 0.f;
+    const void* res = residual ? out : nullptr;
+    const int ld_res = residual ? ld_out : 0;
+    if (path == GEMV) return gemv(x, ldx, w_bf16, K, gamma, eps, res, ld_res, out, ld_out, out_fp32, B, N, K, act, st);
+    if (path == GEMV_NF4) {
+        GemvArgs g;
+        g.x = x; g.ldx = ldx; g.norm_gamma = gamma; g.eps = eps; g.residual = res; g.ld_res = ld_res;
+        g.out = out; g.ld_out = ld_out; g.out_fp32 = out_fp32; g.B = B; g.N = N; g.K = K; g.act = act;
+        return gemv_nf4(g, lin.q.p, lin.a.as<float>(), st);
+    }
+    if (path == SKINNY_FP8) {
+        if (gamma) B2_TRY(rmsnorm_quant_e4m3(x, ldx, gamma, m->xq8.p, K, m->xscale.as<float>(), B, K, eps, st));
+        else B2_TRY(quantize_rows_e4m3(x, ldx, B, K, m->xq8.p, K, m->xscale.as<float>(), st));
+        x = m->xq8.p;
+        ldx = K;
+    } else if (gamma) {
+        B2_TRY(rmsnorm_bf16(x, ldx, gamma, m->xn.p, B, K, eps, st));
+        x = m->xn.p;
+        ldx = K;
+    }
+    if (path == TILE) return gemm(x, ldx, w_bf16, K, nullptr, res, ld_res, out, ld_out, out_fp32, B, N, K, act, st);
+    SkinnyArgs g;
+    g.x = x; g.ldx = ldx; g.W = path == SKINNY_FP8 ? lin.w8.p : w_bf16; g.ldw = K; g.residual = res; g.ld_res = ld_res;
+    g.out = out; g.ld_out = ld_out; g.out_fp32 = out_fp32; g.B = B; g.N = N; g.K = K; g.act = act;
+    g.partial = kv->sk_partial.as<float>(); g.partial_bytes = kv->sk_partial.bytes;
+    g.counters = kv->sk_counters.as<int>();
+    if (path == SKINNY) return gemm_skinny_bf16(g, st);
+    g.w_scale = lin.s8.as<float>(); g.x_scale = m->xscale.as<float>();
+    return gemm_skinny_fp8(g, st);
 }
 
 int decode_nsplit(int B, int H, int max_seq, int ctas_per_sm) {
@@ -416,13 +458,13 @@ int set_llama_layer_weight(b2_model* m, int li, const std::string& s, const char
     for (int j = 0; j < 3; ++j) {
         if (s == names[j]) {
             B2_TRY(expect_shape(key, shape, ndim, h, h));
-            B2_TRY(put(L.wqkv, (size_t)3 * h * h, (size_t)j * h * h, ptr, dt, (int64_t)h * h));
+            B2_TRY(put(L.qkv.w, (size_t)3 * h * h, (size_t)j * h * h, ptr, dt, (int64_t)h * h));
             L.qkv_parts |= 1u << j;
             return 0;
         }
     }
-    if (s == "self_attn.o_proj.weight") { B2_TRY(expect_shape(key, shape, ndim, h, h)); return put(L.wo, (size_t)h * h, 0, ptr, dt, (int64_t)h * h); }
-    if (s == "mlp.down_proj.weight") { B2_TRY(expect_shape(key, shape, ndim, h, I)); return put(L.wd, (size_t)h * I, 0, ptr, dt, (int64_t)h * I); }
+    if (s == "self_attn.o_proj.weight") { B2_TRY(expect_shape(key, shape, ndim, h, h)); return put(L.o.w, (size_t)h * h, 0, ptr, dt, (int64_t)h * h); }
+    if (s == "mlp.down_proj.weight") { B2_TRY(expect_shape(key, shape, ndim, h, I)); return put(L.d.w, (size_t)h * I, 0, ptr, dt, (int64_t)h * I); }
     if (s == "mlp.gate_proj.weight" || s == "mlp.up_proj.weight") {
         B2_TRY(expect_shape(key, shape, ndim, I, h));
         const bool is_gate = s == "mlp.gate_proj.weight";
@@ -430,8 +472,8 @@ int set_llama_layer_weight(b2_model* m, int li, const std::string& s, const char
         B2_TRY(put(tmp, (size_t)I * h, 0, ptr, dt, (int64_t)I * h));
         (is_gate ? L.has_gate : L.has_up) = true;
         if (L.has_gate && L.has_up) {
-            if (L.wgu.p == nullptr) B2_TRY(L.wgu.alloc((size_t)2 * I * h * 2));
-            B2_TRY(interleave_gate_up(L.tmp_gate.p, L.tmp_up.p, L.wgu.p, I, h, 0));
+            if (L.gu.w.p == nullptr) B2_TRY(L.gu.w.alloc((size_t)2 * I * h * 2));
+            B2_TRY(interleave_gate_up(L.tmp_gate.p, L.tmp_up.p, L.gu.w.p, I, h, 0));
             B2_CUDA_CHECK(cudaStreamSynchronize(0));
             L.tmp_gate.free();
             L.tmp_up.free();
@@ -501,6 +543,25 @@ int project_rows(b2_model* m, const void* feats, int rows, void* out, cudaStream
     return 0;
 }
 
+// Captures the kernels fn() enqueues on st and instantiates them as *exec. A capture records launches without running them:
+// g_launch_count is left as it was, and *launches receives the kernel count, which the caller adds on each replay.
+template <typename F>
+int capture_graph(cudaStream_t st, cudaGraphExec_t* exec, int* launches, F fn) {
+    cudaGraph_t graph = nullptr;
+    B2_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+    const unsigned long long launches_before = g_launch_count;
+    const int r = fn();
+    *launches = (int)(g_launch_count - launches_before);
+    g_launch_count = launches_before;
+    cudaError_t e = cudaStreamEndCapture(st, &graph);
+    if (r != 0) { if (graph) cudaGraphDestroy(graph); return r; }
+    B2_CUDA_CHECK(e);
+    e = cudaGraphInstantiate(exec, graph, 0);
+    cudaGraphDestroy(graph);
+    B2_CUDA_CHECK(e);
+    return 0;
+}
+
 // vision tower + projector for one chunk of n <= max_images images: pixels -> out [n*P, hidden]. First call per chunk size runs
 // eagerly (function attributes, driver entry points), the second captures, later ones replay.
 int encode_chunk(b2_model* m, const void* pixels, int n, void* out, cudaStream_t st) {
@@ -528,21 +589,11 @@ int encode_chunk(b2_model* m, const void* pixels, int n, void* out, cudaStream_t
         B2_TRY(project_rows(m, m->v_feats.p, n * m->P, m->enc_out.p, run));
         m->enc_warm[n] = 1;
     } else {
-        if (m->enc_graph[n] == nullptr) {
-            cudaGraph_t graph = nullptr;
-            B2_CUDA_CHECK(cudaStreamBeginCapture(run, cudaStreamCaptureModeThreadLocal));
-            const unsigned long long launches_before = g_launch_count;
-            int r = vit_forward_chunk(m, m->enc_pixels.p, n, m->v_feats.p, run);
-            if (r == 0) r = project_rows(m, m->v_feats.p, n * m->P, m->enc_out.p, run);
-            m->enc_launches = (int)(g_launch_count - launches_before);
-            g_launch_count = launches_before;  // capture records launches, it does not run them
-            cudaError_t e = cudaStreamEndCapture(run, &graph);
-            if (r != 0) { if (graph) cudaGraphDestroy(graph); return r; }
-            B2_CUDA_CHECK(e);
-            e = cudaGraphInstantiate(&m->enc_graph[n], graph, 0);
-            cudaGraphDestroy(graph);
-            B2_CUDA_CHECK(e);
-        }
+        if (m->enc_graph[n] == nullptr)
+            B2_TRY(capture_graph(run, &m->enc_graph[n], &m->enc_launches, [&] {
+                B2_TRY(vit_forward_chunk(m, m->enc_pixels.p, n, m->v_feats.p, run));
+                return project_rows(m, m->v_feats.p, n * m->P, m->enc_out.p, run);
+            }));
         B2_CUDA_CHECK(cudaGraphLaunch(m->enc_graph[n], run));
         g_launch_count += (unsigned long long)m->enc_launches;
     }
@@ -559,35 +610,14 @@ int decode_step_launch(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     const b2_model_desc& d = m->d;
     const int h = d.hidden, I = d.inter, H = d.heads, V = d.vocab;
     const int nsplit = decode_nsplit(B, H, kv->max_seq, kv->e4m3() ? decode_attn_e4m3_ctas_per_sm() : decode_attn_ctas_per_sm());
+    const DecodePlan plan = decode_plan(m, kv, B);
+    const DecodePath p = plan.layer;
     B2_TRY(embed_tokens(kv->tok.as<int32_t>(), m->embed.p, m->x.p, B, h, V, m->err_dev, st));
-    // batch <= 8: tensor-core GEMV kernels (falls back to the skinny-M wgmma GEMM when the activations do not fit smem)
-    // batch 7..128: swap-AB stream-K GEMM (weights streamed once, all SMs busy); otherwise GEMV kernels (B <= 8) or
-    // the tile GEMM
-    // NF4 model: gemv_nf4 at batch <= 8; otherwise each layer is dequantised into the scratch in front of the paths below
-    const bool small4 = use_gemv_nf4(m, B);
-    const bool sk = !small4 && use_skinny(kv, B);
-    const bool small = !m->nf4 && !sk && B <= 8 && gemv_fits(B, h, I, ACT_NONE) && gemv_fits(B, 2 * I, h, ACT_SWIGLU) &&
-                       gemv_fits(B, 3 * h, h, ACT_NONE) && gemv_fits(B, V, h, ACT_NONE);
-    const bool f8 = sk && m->fp8_decode;  // e4m3 weights x e4m3 activations through the same stream-K GEMM
     for (int l = 0; l < d.layers; ++l) {
         LlamaLayer& L = m->ll[l];
         LayerW lw = {};
-        if (!small4) B2_TRY(layer_weights(m, l, &lw, st));
-        if (small4) {
-            B2_TRY(gemv4(m->x.p, h, L.q_qkv, L.a_qkv, L.ln1.p, d.rms_eps, nullptr, 0, m->qkv.p, 3 * h, B, 3 * h, h, ACT_NONE, st));
-        } else if (f8) {
-            B2_TRY(rmsnorm_quant_e4m3(m->x.p, h, L.ln1.p, m->xq8.p, h, m->xscale.as<float>(), B, h, d.rms_eps, st));
-            B2_TRY(skinny8(m, kv, L.wqkv8.p, L.s_qkv.as<float>(), nullptr, 0, m->qkv.p, 3 * h, 0, B, 3 * h, h, ACT_NONE, st));
-        } else if (small) {
-            B2_TRY(gemv(m->x.p, h, L.wqkv.p, h, L.ln1.p, d.rms_eps, nullptr, 0, m->qkv.p, 3 * h, 0, B, 3 * h, h,
-                        ACT_NONE, st));
-        } else if (sk) {
-            B2_TRY(rmsnorm_bf16(m->x.p, h, L.ln1.p, m->xn.p, B, h, d.rms_eps, st));
-            B2_TRY(skinny(kv, m->xn.p, h, lw.wqkv, h, nullptr, 0, m->qkv.p, 3 * h, 0, B, 3 * h, h, ACT_NONE, st));
-        } else {
-            B2_TRY(rmsnorm_bf16(m->x.p, h, L.ln1.p, m->xn.p, B, h, d.rms_eps, st));
-            B2_TRY(gemm(m->xn.p, h, lw.wqkv, h, nullptr, nullptr, 0, m->qkv.p, 3 * h, 0, B, 3 * h, h, ACT_NONE, st));
-        }
+        if (p != GEMV_NF4) B2_TRY(layer_weights(m, l, &lw, st));
+        B2_TRY(decode_linear(m, kv, p, L.qkv, lw.wqkv, m->x.p, h, L.ln1.p, false, m->qkv.p, 3 * h, 0, B, 3 * h, h, ACT_NONE, st));
         DecodeAttnArgs da;
         da.qkv = m->qkv.p;
         da.kcache = kv->k_layer(l);
@@ -606,59 +636,14 @@ int decode_step_launch(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
         } else {
             B2_TRY(decode_attn_bf16(da, st));
         }
-        if (small4) {
-            B2_TRY(gemv4(m->attn.p, h, L.q_o, L.a_o, nullptr, 0.f, m->x.p, h, m->x.p, h, B, h, h, ACT_NONE, st));
-            B2_TRY(gemv4(m->x.p, h, L.q_gu, L.a_gu, L.ln2.p, d.rms_eps, nullptr, 0, m->act.p, I, B, 2 * I, h, ACT_SWIGLU, st));
-            B2_TRY(gemv4(m->act.p, I, L.q_d, L.a_d, nullptr, 0.f, m->x.p, h, m->x.p, h, B, h, I, ACT_NONE, st));
-        } else if (f8) {
-            B2_TRY(quantize_rows_e4m3(m->attn.p, h, B, h, m->xq8.p, h, m->xscale.as<float>(), st));
-            B2_TRY(skinny8(m, kv, L.wo8.p, L.s_o.as<float>(), m->x.p, h, m->x.p, h, 0, B, h, h, ACT_NONE, st));
-            B2_TRY(rmsnorm_quant_e4m3(m->x.p, h, L.ln2.p, m->xq8.p, h, m->xscale.as<float>(), B, h, d.rms_eps, st));
-            B2_TRY(skinny8(m, kv, L.wgu8.p, L.s_gu.as<float>(), nullptr, 0, m->act.p, I, 0, B, 2 * I, h, ACT_SWIGLU, st));
-            B2_TRY(quantize_rows_e4m3(m->act.p, I, B, I, m->xq8.p, I, m->xscale.as<float>(), st));
-            B2_TRY(skinny8(m, kv, L.wd8.p, L.s_d.as<float>(), m->x.p, h, m->x.p, h, 0, B, h, I, ACT_NONE, st));
-        } else if (small) {
-            B2_TRY(gemv(m->attn.p, h, L.wo.p, h, nullptr, 0.f, m->x.p, h, m->x.p, h, 0, B, h, h, ACT_NONE, st));
-            B2_TRY(gemv(m->x.p, h, L.wgu.p, h, L.ln2.p, d.rms_eps, nullptr, 0, m->act.p, I, 0, B, 2 * I, h,
-                        ACT_SWIGLU, st));
-            B2_TRY(gemv(m->act.p, I, L.wd.p, I, nullptr, 0.f, m->x.p, h, m->x.p, h, 0, B, h, I, ACT_NONE, st));
-        } else if (sk) {
-            B2_TRY(skinny(kv, m->attn.p, h, lw.wo, h, m->x.p, h, m->x.p, h, 0, B, h, h, ACT_NONE, st));
-            B2_TRY(rmsnorm_bf16(m->x.p, h, L.ln2.p, m->xn.p, B, h, d.rms_eps, st));
-            B2_TRY(skinny(kv, m->xn.p, h, lw.wgu, h, nullptr, 0, m->act.p, I, 0, B, 2 * I, h, ACT_SWIGLU, st));
-            B2_TRY(skinny(kv, m->act.p, I, lw.wd, I, m->x.p, h, m->x.p, h, 0, B, h, I, ACT_NONE, st));
-        } else {
-            B2_TRY(gemm(m->attn.p, h, lw.wo, h, nullptr, m->x.p, h, m->x.p, h, 0, B, h, h, ACT_NONE, st));
-            B2_TRY(rmsnorm_bf16(m->x.p, h, L.ln2.p, m->xn.p, B, h, d.rms_eps, st));
-            B2_TRY(gemm(m->xn.p, h, lw.wgu, h, nullptr, nullptr, 0, m->act.p, I, 0, B, 2 * I, h, ACT_SWIGLU, st));
-            B2_TRY(gemm(m->act.p, I, lw.wd, I, nullptr, m->x.p, h, m->x.p, h, 0, B, h, I, ACT_NONE, st));
-        }
+        B2_TRY(decode_linear(m, kv, p, L.o, lw.wo, m->attn.p, h, nullptr, true, m->x.p, h, 0, B, h, h, ACT_NONE, st));
+        B2_TRY(decode_linear(m, kv, p, L.gu, lw.wgu, m->x.p, h, L.ln2.p, false, m->act.p, I, 0, B, 2 * I, h, ACT_SWIGLU, st));
+        B2_TRY(decode_linear(m, kv, p, L.d, lw.wd, m->act.p, I, nullptr, true, m->x.p, h, 0, B, h, I, ACT_NONE, st));
     }
-    if (f8) {
-        B2_TRY(rmsnorm_quant_e4m3(m->x.p, h, m->final_norm.p, m->xq8.p, h, m->xscale.as<float>(), B, h, d.rms_eps, st));
-        B2_TRY(skinny8(m, kv, m->lm_head8.p, m->s_head.as<float>(), nullptr, 0, m->logits.p, V, 1, B, V, h, ACT_NONE, st));
-    } else if (small || (small4 && gemv_fits(B, V, h, ACT_NONE))) {
-        B2_TRY(gemv(m->x.p, h, m->lm_head.p, h, m->final_norm.p, d.rms_eps, nullptr, 0, m->logits.p, V, 1, B, V, h,
-                    ACT_NONE, st));
-    } else if (sk) {
-        B2_TRY(rmsnorm_bf16(m->x.p, h, m->final_norm.p, m->xn.p, B, h, d.rms_eps, st));
-        B2_TRY(skinny(kv, m->xn.p, h, m->lm_head.p, h, nullptr, 0, m->logits.p, V, 1, B, V, h, ACT_NONE, st));
-    } else {
-        B2_TRY(rmsnorm_bf16(m->x.p, h, m->final_norm.p, m->xn.p, B, h, d.rms_eps, st));
-        B2_TRY(gemm(m->xn.p, h, m->lm_head.p, h, nullptr, nullptr, 0, m->logits.p, V, 1, B, V, h, ACT_NONE, st));
-    }
-    {   // A/B switch for measurements: the separate tail (argmax + store_token + 2 x add_i32), greedy only, no host ring
-        const char* e = getenv("B2_SAMPLE_LEGACY");
-        if (e != nullptr && e[0] == '1' && kv->samp_host.do_sample == 0 && kv->samp_host.tag == 0 && kv->samp_host.per_row == 0) {
-            B2_TRY(argmax_f32(m->logits.as<float>(), B, V, kv->tok.as<int32_t>(), st));
-            B2_TRY(store_token(kv->tok.as<int32_t>(), kv->out_tokens.as<int32_t>(), kv->step_counter.as<int32_t>(), B, st));
-            B2_TRY(add_i32(kv->step_counter.as<int32_t>(), 1, 1, st));
-            B2_TRY(add_i32(kv->len_dev.as<int32_t>(), B, 1, st));
-            return 0;
-        }
-    }
+    B2_TRY(decode_linear(m, kv, plan.head, m->head, m->head.w.p, m->x.p, h, m->final_norm.p, false, m->logits.p, V, 1, B, V, h,
+                         ACT_NONE, st));
     // argmax or temperature/top-k/top-p draw (device-resident SampleState), token feedback, host-ring publication and the
-    // step / cache-length counters in ONE launch (was: argmax + store_token + 2 x add_i32)
+    // step / cache-length counters in one launch
     B2_TRY(sample_publish(m->logits.as<float>(), V, B, kv->sstate.as<SampleState>(), kv->rows_dev.as<RowState>(), kv->tok.as<int32_t>(),
                           kv->out_tokens.as<int32_t>(), kv->step_counter.as<int32_t>(), kv->len_dev.as<int32_t>(),
                           kv->ring_dev, kv->ring_cap, SP_SELECT | SP_WRITE_OUT | SP_BUMP, 0, st));
@@ -710,7 +695,7 @@ int decode_step_mega(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     p.L = d.layers; p.h = d.hidden; p.I = d.inter; p.H = d.heads; p.V = d.vocab; p.B = B; p.Smax = kv->pitch;
     int ns = (num_sms() * 16) / (B * d.heads);
     p.nsplit = ns < 1 ? 1 : (ns > 64 ? 64 : ns);
-    p.embed = m->embed.as<bf16>(); p.final_norm = m->final_norm.as<bf16>(); p.lm_head = m->lm_head.as<bf16>();
+    p.embed = m->embed.as<bf16>(); p.final_norm = m->final_norm.as<bf16>(); p.lm_head = m->head.w.as<bf16>();
     p.tok = kv->tok.as<int32_t>(); p.cur_len = kv->len_dev.as<int32_t>();
     p.out_tokens = kv->out_tokens.as<int32_t>(); p.step_counter = kv->step_counter.as<int32_t>();
     p.x = m->x.as<bf16>(); p.qkv = m->qkv.as<bf16>(); p.attn = m->attn.as<bf16>(); p.act = m->act.as<bf16>();
@@ -784,32 +769,11 @@ int decode_step_run(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     }
     if (kv->graph == nullptr || kv->graph_B != B) {
         if (kv->graph) { cudaGraphExecDestroy(kv->graph); kv->graph = nullptr; }
-        cudaGraph_t graph = nullptr;
-        B2_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-        const unsigned long long launches_before = g_launch_count;
-        int r = decode_step_launch(m, kv, B, st);
-        g_launch_count = launches_before;  // capture records launches, it does not run them
-        cudaError_t e = cudaStreamEndCapture(st, &graph);
-        if (r != 0) { if (graph) cudaGraphDestroy(graph); return r; }
-        B2_CUDA_CHECK(e);
-        e = cudaGraphInstantiate(&kv->graph, graph, 0);
-        cudaGraphDestroy(graph);
-        B2_CUDA_CHECK(e);
+        B2_TRY(capture_graph(st, &kv->graph, &kv->graph_launches, [&] { return decode_step_launch(m, kv, B, st); }));
         kv->graph_B = B;
     }
     B2_CUDA_CHECK(cudaGraphLaunch(kv->graph, st));
-    // kernels per step: embed + L*(qkv, attn, o, gate/up, down [+2 norms when B>8]) + head(+norm) + sample_publish
-    // (NF4: 5 per layer with gemv_nf4, otherwise the dequantisation of the layer in front of the 7)
-    if (m->nf4) {
-        const bool small4 = use_gemv_nf4(m, B);
-        const bool head_gemv = small4 && gemv_fits(B, m->d.vocab, m->d.hidden, ACT_NONE);
-        g_launch_count += 1 + (unsigned long long)m->d.layers * (small4 ? 5 : 8) + (head_gemv ? 1 : 2) + 1;
-        return 0;
-    }
-    const bool small = !use_skinny(kv, B) && B <= 8 && gemv_fits(B, m->d.hidden, m->d.inter, ACT_NONE) &&
-                       gemv_fits(B, m->d.vocab, m->d.hidden, ACT_NONE);
-    const int per_layer = small ? 5 : ((m->fp8_decode && use_skinny(kv, B)) ? 9 : 7);
-    g_launch_count += 1 + (unsigned long long)m->d.layers * per_layer + (small ? 1 : 2) + 1;
+    g_launch_count += (unsigned long long)kv->graph_launches;
     return 0;
 }
 
@@ -911,7 +875,7 @@ int b2_model_set_weight(b2_model* m, const char* hf_key, const void* ptr, const 
         r = put(m->final_norm, h, 0, ptr, dtype, h);
     } else if (k == "lm_head.weight") {
         B2_TRY(expect_shape(hf_key, shape, ndim, V, h));
-        r = put(m->lm_head, (size_t)V * h, 0, ptr, dtype, (int64_t)V * h);
+        r = put(m->head.w, (size_t)V * h, 0, ptr, dtype, (int64_t)V * h);
     } else if (m->nf4 && (k == "model.mm_projector.0.weight" || k == "model.mm_projector.2.weight")) {
         set_error("set_weight(%s): the projector of this model holds its NF4 w_hat (b2_model_enable_nf4); it cannot be reloaded", hf_key);
         return -1;
@@ -961,10 +925,10 @@ int b2_model_finalize(b2_model* m) {
     }
     need(m->p0_w, "mm_projector.0.weight"); need(m->p0_b, "mm_projector.0.bias");
     need(m->p2_w, "mm_projector.2.weight"); need(m->p2_b, "mm_projector.2.bias");
-    need(m->embed, "embed_tokens"); need(m->final_norm, "model.norm"); need(m->lm_head, "lm_head");
+    need(m->embed, "embed_tokens"); need(m->final_norm, "model.norm"); need(m->head.w, "lm_head");
     for (size_t i = 0; i < m->ll.size(); ++i) {
         LlamaLayer& L = m->ll[i];
-        const DevBuf* bs[6] = {&L.ln1, &L.wqkv, &L.wo, &L.ln2, &L.wgu, &L.wd};
+        const DevBuf* bs[6] = {&L.ln1, &L.qkv.w, &L.o.w, &L.ln2, &L.gu.w, &L.d.w};
         for (int j = 0; j < 6; ++j)
             if (bs[j]->p == nullptr) { char t[64]; snprintf(t, sizeof t, "layers.%zu.#%d", i, j); need(*bs[j], t); }
     }
@@ -1034,20 +998,19 @@ int b2_model_destroy(b2_model* m) {
     if (m->enc_fork) cudaEventDestroy(m->enc_fork);
     if (m->enc_join) cudaEventDestroy(m->enc_join);
     DevBuf* top[] = {&m->patch_w, &m->cls, &m->pos, &m->pre_g, &m->pre_b, &m->p0_w, &m->p0_b, &m->p2_w, &m->p2_b,
-                     &m->embed, &m->final_norm, &m->lm_head, &m->v_col, &m->v_patch, &m->v_hidden, &m->v_xn,
+                     &m->embed, &m->final_norm, &m->v_col, &m->v_patch, &m->v_hidden, &m->v_xn,
                      &m->v_qkv, &m->v_attn, &m->v_mlp, &m->v_feats, &m->p_mid, &m->p_done, &m->enc_pixels, &m->enc_out, &m->x, &m->xn, &m->qkv, &m->attn,
-                     &m->act, &m->last_idx, &m->chunk_pos, &m->xlast, &m->logits, &m->splice_idx, &m->lm_head8, &m->s_head, &m->xq8, &m->xscale,
+                     &m->act, &m->last_idx, &m->chunk_pos, &m->xlast, &m->logits, &m->splice_idx, &m->xq8, &m->xscale,
                      &m->kstage, &m->vstage, &m->nf4_scratch};
     for (DevBuf* b : top) b->free();
+    m->head.free();
     for (VitLayer& L : m->vit) {
         DevBuf* bs[12] = {&L.ln1_g, &L.ln1_b, &L.wqkv, &L.bqkv, &L.wo, &L.bo, &L.ln2_g, &L.ln2_b, &L.w1, &L.b1, &L.w2, &L.b2};
         for (DevBuf* b : bs) b->free();
     }
     for (LlamaLayer& L : m->ll) {
-        DevBuf* bs[24] = {&L.ln1, &L.wqkv, &L.wo, &L.ln2, &L.wgu, &L.wd, &L.tmp_gate, &L.tmp_up,
-                          &L.wqkv8, &L.wo8, &L.wgu8, &L.wd8, &L.s_qkv, &L.s_o, &L.s_gu, &L.s_d,
-                          &L.q_qkv, &L.a_qkv, &L.q_o, &L.a_o, &L.q_gu, &L.a_gu, &L.q_d, &L.a_d};
-        for (DevBuf* b : bs) b->free();
+        for (DevBuf* b : {&L.ln1, &L.ln2, &L.tmp_gate, &L.tmp_up}) b->free();
+        for (Linear* lin : L.linears()) lin->free();
     }
     delete m;
     return 0;
@@ -1065,18 +1028,18 @@ int b2_model_enable_fp8_decode(b2_model* m) {
     const b2_model_desc& d = m->d;
     const int h = d.hidden, I = d.inter, V = d.vocab;
     B2_CHECK_ARG(h % 16 == 0 && I % 16 == 0, "b2_model_enable_fp8_decode: hidden/inter must be multiples of 16");
-    auto quant = [&](DevBuf& w, int N, int K, DevBuf& w8, DevBuf& sc) -> int {
-        B2_TRY(w8.alloc((size_t)N * K));
-        B2_TRY(sc.alloc((size_t)N * sizeof(float)));
-        return quantize_rows_e4m3(w.p, K, N, K, w8.p, K, sc.as<float>(), nullptr);
+    // gate/up rows stay block-64 interleaved; its scales follow the physical rows
+    auto quant = [&](Linear& lin, int N, int K) -> int {
+        B2_TRY(lin.w8.alloc((size_t)N * K));
+        B2_TRY(lin.s8.alloc((size_t)N * sizeof(float)));
+        return quantize_rows_e4m3(lin.w.p, K, N, K, lin.w8.p, K, lin.s8.as<float>(), nullptr);
     };
+    const auto sh = layer_shapes(d);
     for (LlamaLayer& L : m->ll) {
-        B2_TRY(quant(L.wqkv, 3 * h, h, L.wqkv8, L.s_qkv));
-        B2_TRY(quant(L.wo, h, h, L.wo8, L.s_o));
-        B2_TRY(quant(L.wgu, 2 * I, h, L.wgu8, L.s_gu));  // rows stay block-64 interleaved; scales follow the physical rows
-        B2_TRY(quant(L.wd, h, I, L.wd8, L.s_d));
+        const auto lin = L.linears();
+        for (int i = 0; i < 4; ++i) B2_TRY(quant(*lin[i], sh[i].N, sh[i].K));
     }
-    B2_TRY(quant(m->lm_head, V, h, m->lm_head8, m->s_head));
+    B2_TRY(quant(m->head, V, h));
     const int mb = d.max_batch > 128 ? 128 : d.max_batch;
     B2_TRY(m->xq8.alloc((size_t)mb * (h > I ? h : I)));
     B2_TRY(m->xscale.alloc((size_t)mb * sizeof(float)));
@@ -1098,17 +1061,20 @@ int b2_model_enable_nf4(b2_model* m) {
     B2_CHECK_ARG(m->kv_live.load() == 0, "b2_model_enable_nf4: %d KV cache(s) exist; enable NF4 before creating any (the megakernel "
                  "tables of existing caches point at the bf16 weights)", m->kv_live.load());
     const b2_model_desc& d = m->d;
-    const int h = d.hidden, I = d.inter, D = d.vit_hidden;
-    auto quant = [&](const DevBuf& w, int N, int K, DevBuf& q, DevBuf& a) -> int {
-        B2_TRY(q.alloc((size_t)N * K / 2));
-        B2_TRY(a.alloc((size_t)N * (K / 64) * sizeof(float)));
-        return quantize_nf4(w.p, K, N, K, q.p, a.as<float>(), 1, nullptr);
+    const int h = d.hidden, D = d.vit_hidden;
+    auto quant = [&](Linear& lin, int N, int K) -> int {
+        B2_TRY(lin.q.alloc((size_t)N * K / 2));
+        B2_TRY(lin.a.alloc((size_t)N * (K / 64) * sizeof(float)));
+        return quantize_nf4(lin.w.p, K, N, K, lin.q.p, lin.a.as<float>(), 1, nullptr);
     };
+    const auto sh = layer_shapes(d);
+    size_t scratch = 0;  // elements of one dequantised layer
+    for (const LinearShape& s : sh) scratch += (size_t)s.N * s.K;
     int r = 0;
     for (LlamaLayer& L : m->ll) {
-        if ((r = quant(L.wqkv, 3 * h, h, L.q_qkv, L.a_qkv)) != 0 || (r = quant(L.wo, h, h, L.q_o, L.a_o)) != 0 ||
-            (r = quant(L.wgu, 2 * I, h, L.q_gu, L.a_gu)) != 0 || (r = quant(L.wd, h, I, L.q_d, L.a_d)) != 0)
-            break;
+        const auto lin = L.linears();
+        for (int i = 0; i < 4 && r == 0; ++i) r = quant(*lin[i], sh[i].N, sh[i].K);
+        if (r != 0) break;
     }
     // projector: w -> codes (canonical) -> w_hat, in place
     DevBuf pq, pa;
@@ -1125,7 +1091,7 @@ int b2_model_enable_nf4(b2_model* m) {
         return 0;
     };
     DevBuf p0_hat, p2_hat;
-    if (r == 0) r = m->nf4_scratch.alloc(((size_t)4 * h * h + (size_t)3 * I * h) * 2);
+    if (r == 0) r = m->nf4_scratch.alloc(scratch * 2);
     if (r == 0 && cudaDeviceSynchronize() != cudaSuccess) { set_error("b2_model_enable_nf4: quantisation failed: %s", cudaGetErrorString(cudaGetLastError())); r = -2; }
     if (r == 0) r = roundtrip(m->p0_w, h, D, p0_hat);
     if (r == 0) r = roundtrip(m->p2_w, h, h, p2_hat);
@@ -1133,7 +1099,7 @@ int b2_model_enable_nf4(b2_model* m) {
     pa.free();
     if (r != 0) {  // nothing of the model has changed yet
         for (LlamaLayer& L : m->ll)
-            for (DevBuf* b : {&L.q_qkv, &L.a_qkv, &L.q_o, &L.a_o, &L.q_gu, &L.a_gu, &L.q_d, &L.a_d}) b->free();
+            for (Linear* lin : L.linears()) { lin->q.free(); lin->a.free(); }
         m->nf4_scratch.free();
         p0_hat.free();
         p2_hat.free();
@@ -1144,7 +1110,7 @@ int b2_model_enable_nf4(b2_model* m) {
     p0_hat.free();  // now the bf16 originals
     p2_hat.free();
     for (LlamaLayer& L : m->ll)
-        for (DevBuf* b : {&L.wqkv, &L.wo, &L.wgu, &L.wd}) b->free();
+        for (Linear* lin : L.linears()) lin->w.free();
     m->nf4 = true;
     return 0;
 }
@@ -1154,15 +1120,16 @@ int64_t b2_model_weight_bytes(b2_model* m) {
     std::lock_guard<std::mutex> lk(m->mu);
     size_t n = 0;
     for (const DevBuf* b : {&m->patch_w, &m->cls, &m->pos, &m->pre_g, &m->pre_b, &m->p0_w, &m->p0_b, &m->p2_w, &m->p2_b, &m->embed,
-                            &m->final_norm, &m->lm_head, &m->lm_head8, &m->s_head})
+                            &m->final_norm})
         n += b->bytes;
+    n += m->head.bytes();
     for (const VitLayer& L : m->vit)
         for (const DevBuf* b : {&L.ln1_g, &L.ln1_b, &L.wqkv, &L.bqkv, &L.wo, &L.bo, &L.ln2_g, &L.ln2_b, &L.w1, &L.b1, &L.w2, &L.b2})
             n += b->bytes;
-    for (const LlamaLayer& L : m->ll)
-        for (const DevBuf* b : {&L.ln1, &L.wqkv, &L.wo, &L.ln2, &L.wgu, &L.wd, &L.wqkv8, &L.wo8, &L.wgu8, &L.wd8, &L.s_qkv, &L.s_o,
-                                &L.s_gu, &L.s_d, &L.q_qkv, &L.a_qkv, &L.q_o, &L.a_o, &L.q_gu, &L.a_gu, &L.q_d, &L.a_d})
-            n += b->bytes;
+    for (LlamaLayer& L : m->ll) {
+        n += L.ln1.bytes + L.ln2.bytes;
+        for (const Linear* lin : L.linears()) n += lin->bytes();
+    }
     return (int64_t)n;
 }
 
@@ -1209,8 +1176,8 @@ int b2_kv_create_ex(b2_model* m, int max_batch, int max_seq, int kv_dtype, b2_kv
         std::vector<MegaLayer> tbl(m->d.layers);
         for (int l = 0; l < m->d.layers; ++l) {
             LlamaLayer& L = m->ll[l];
-            tbl[l].ln1 = L.ln1.as<bf16>(); tbl[l].wqkv = L.wqkv.as<bf16>(); tbl[l].wo = L.wo.as<bf16>();
-            tbl[l].ln2 = L.ln2.as<bf16>(); tbl[l].wgu = L.wgu.as<bf16>(); tbl[l].wd = L.wd.as<bf16>();
+            tbl[l].ln1 = L.ln1.as<bf16>(); tbl[l].wqkv = L.qkv.w.as<bf16>(); tbl[l].wo = L.o.w.as<bf16>();
+            tbl[l].ln2 = L.ln2.as<bf16>(); tbl[l].wgu = L.gu.w.as<bf16>(); tbl[l].wd = L.d.w.as<bf16>();
             tbl[l].kcache = reinterpret_cast<bf16*>(kv->k_layer(l));  // read by the megakernel, which a bf16 cache alone reaches
             tbl[l].vcache = reinterpret_cast<bf16*>(kv->v_layer(l));
         }
@@ -1227,16 +1194,16 @@ int b2_kv_create_ex(b2_model* m, int max_batch, int max_seq, int kv_dtype, b2_kv
         b2_kv_destroy(kv);
         return r;
     }
-    if (max_batch >= 3 && max_batch <= 128) {
-        const int h = m->d.hidden, I = m->d.inter, V = m->d.vocab;
+    if (max_batch >= 7 && max_batch <= 128) {  // the batches use_skinny takes
         size_t ws = 0;
-        const int shapes[5][2] = {{3 * h, h}, {h, h}, {2 * I, h}, {h, I}, {V, h}};
         int nmax = 0;
-        for (auto& sh : shapes) {
-            const size_t b = gemm_skinny_workspace_bytes(max_batch, sh[0], sh[1]);
+        auto fit = [&](int N, int K) {
+            const size_t b = gemm_skinny_workspace_bytes(max_batch, N, K);
             ws = b > ws ? b : ws;
-            nmax = sh[0] > nmax ? sh[0] : nmax;
-        }
+            nmax = N > nmax ? N : nmax;
+        };
+        for (const LinearShape& sh : layer_shapes(m->d)) fit(sh.N, sh.K);
+        fit(m->d.vocab, m->d.hidden);
         if ((r = kv->sk_partial.alloc(ws)) != 0 || (r = kv->sk_counters.alloc(gemm_skinny_counter_bytes(nmax))) != 0) {
             b2_kv_destroy(kv);
             return r;
@@ -1537,12 +1504,12 @@ int b2_prefill_at(b2_model* m, b2_kv* kv, const void* embeds, const int32_t* sta
         // only the last valid position per sample feeds generation (the reference computes lm_head on all S)
         B2_TRY(rmsnorm_gather_bf16(m->x.p, m->last_idx.as<int32_t>(), m->final_norm.p, m->xlast.p, B, h, d.rms_eps, st));
         if (B <= 8 && gemv_fits(B, V, h, ACT_NONE))
-            B2_TRY(gemv(m->xlast.p, h, m->lm_head.p, h, nullptr, 0.f, nullptr, 0, logits_out, V, 1, B, V, h, ACT_NONE, st));
+            B2_TRY(gemv(m->xlast.p, h, m->head.w.p, h, nullptr, 0.f, nullptr, 0, logits_out, V, 1, B, V, h, ACT_NONE, st));
         else
-            B2_TRY(gemm(m->xlast.p, h, m->lm_head.p, h, nullptr, nullptr, 0, logits_out, V, 1, B, V, h, ACT_NONE, st));
+            B2_TRY(gemm(m->xlast.p, h, m->head.w.p, h, nullptr, nullptr, 0, logits_out, V, 1, B, V, h, ACT_NONE, st));
     } else if (logits_mode == B2_LOGITS_ALL) {
         B2_TRY(rmsnorm_bf16(m->x.p, h, m->final_norm.p, m->xn.p, T, h, d.rms_eps, st));
-        B2_TRY(gemm(m->xn.p, h, m->lm_head.p, h, nullptr, nullptr, 0, logits_out, V, 1, T, V, h, ACT_NONE, st));
+        B2_TRY(gemm(m->xn.p, h, m->head.w.p, h, nullptr, nullptr, 0, logits_out, V, 1, T, V, h, ACT_NONE, st));
     }
     return ws_leave(m, st);
 }

@@ -2,7 +2,7 @@
 batch size under environment variants read at graph-capture time; also the HOST time of the enqueueing call (a replayed
 graph returns in ~N x 20 us, launch-by-launch enqueueing takes as long as the GPU work).
 
-    python scripts/decode_ab.py --batches 8,32 --variants "default;B2_SAMPLE_LEGACY=1;B2_DECODE_SKINNY=0"
+    python scripts/decode_ab.py --batches 8,32 --variants "default;B2_DECODE_SKINNY=0"
 """
 import argparse
 import json
@@ -25,7 +25,7 @@ def main():
     ap.add_argument("--model", default="7b")
     ap.add_argument("--batches", default="8,32")
     ap.add_argument("--new", type=int, default=64)
-    ap.add_argument("--variants", default="default;B2_SAMPLE_LEGACY=1")
+    ap.add_argument("--variants", default="default;B2_DECODE_SKINNY=0")
     ap.add_argument("--out", default=os.devnull, help="also append every result line to this file")
     a = ap.parse_args()
     from llava import _b2
