@@ -72,6 +72,27 @@ typedef struct b2_sampling {
     unsigned long long seed;  /* Philox key; draw t of row b is a pure function of (logits, seed, t, b) */
 } b2_sampling;
 
+/* History-aware logits processing of one row, applied before token selection in HF 5.5's order (GenerationMixin
+ * _get_logits_processor): repetition penalty -> no-repeat n-gram -> min_length / min_new_tokens -> temperature -> top-k -> top-p.
+ * The row's history is prompt_ids[0, prompt_len) (device int64, the caller's prompt row as passed, IMAGE_TOKEN_INDEX
+ * placeholders and pad ids included) followed by the tokens generated so far.
+ *   repetition_penalty  p > 0, 1 = off: every distinct history id in [0, vocab) gets x < 0 ? x * p : x / p (IEEE fp32)
+ *   no_repeat_ngram_size n >= 0, 0 = off: every history n-gram whose first n-1 ids equal the last n-1 ids bans its last id
+ *                        (-inf) unless that id is outside [0, vocab); nothing is banned while history length + 1 < n
+ *   min_generated        eos_ids[0, n_eos) get -inf while fewer than min_generated tokens were generated
+ *                        (max(min_new_tokens, min_length - prompt_len) for HF's two processors); no effect with n_eos == 0
+ * A row with every processor off is selected exactly as without this struct. The pointed-to ids are read by the call's
+ * stream work only (they must stay valid until it has run). */
+typedef struct b2_logits_proc {
+    float repetition_penalty;
+    int32_t no_repeat_ngram_size;
+    int32_t min_generated;
+    int32_t n_eos;               /* 0..8 */
+    int32_t eos_ids[8];
+    const int64_t* prompt_ids;   /* device */
+    int32_t prompt_len;
+} b2_logits_proc;
+
 /* ---- lifecycle ------------------------------------------------------------------------------------------ */
 int b2_init(int device);                 /* cudaSetDevice + capability check (needs sm_90) */
 const char* b2_last_error(void);         /* thread-local message of the last failing call */
@@ -203,6 +224,14 @@ int b2_argmax(const float* logits, int B, int V, int32_t* out, void* stream);
  *                     timeout_ms <= 0 waits forever; -3 on timeout, -2 if the device faulted.
  * Steps that were queued past the point where the host decides to stop simply run to completion (rows never interact). */
 int b2_stream_begin(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sampling, void* stream);
+/* b2_stream_begin with logits processors: proc[b] (nullable = all off) for sample b. Token 0 is chosen from the processed
+ * prefill logits over the prompt history; every later step of the generation processes against the history kept on the
+ * device (prompt, then each chosen token). The cache's processing state is allocated by the first call that turns a processor
+ * on (b2_kv_bytes does not count it). b2_stream_begin, b2_batch_begin, b2_decode_step, b2_decode_greedy and b2_beam_step turn
+ * every row's processors off. -1 for repetition_penalty <= 0, a negative n-gram size, n_eos outside [0, 8] or a prompt longer
+ * than the cache's max_seq. */
+int b2_stream_begin_ex(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sampling, const b2_logits_proc* proc,
+                       void* stream);
 int b2_stream_enqueue(b2_model* m, b2_kv* kv, int n_steps, void* stream);
 int b2_stream_wait(b2_kv* kv, int index, int32_t* tokens_host, int timeout_ms);
 
@@ -215,6 +244,10 @@ int b2_stream_wait(b2_kv* kv, int index, int32_t* tokens_host, int timeout_ms);
  * slot. Token selection is per slot: greedy or temperature/top-k/top-p with the slot's own Philox stream. */
 int b2_batch_begin(b2_model* m, b2_kv* kv, int B, void* stream);
 int b2_batch_set_row(b2_model* m, b2_kv* kv, int slot, int active, const b2_sampling* sampling, int first_token, void* stream);
+/* b2_batch_set_row with the slot's logits processors (nullable = off): its history is proc's prompt ids followed by first_token
+ * (chosen by the caller, e.g. with b2_op_sample_ex over the same prompt). A freed slot's processors are turned off. */
+int b2_batch_set_row_ex(b2_model* m, b2_kv* kv, int slot, int active, const b2_sampling* sampling, const b2_logits_proc* proc,
+                        int first_token, void* stream);
 
 /* Beam search (generate(num_beams > 1): HF GenerationMixin._beam_search of the installed transformers 5.5, as the reference's eval
  * scripts call it with --num_beams, llava/eval/run_llava.py:121,153). The B*nb running beams of B samples live in cache slots;
@@ -345,6 +378,10 @@ int b2_op_preprocess_clip(const b2_preprocess_plan* plan, void* stream);
 /* one selection per row from fp32 logits [B,V] (csrc/sampling.cu): out_tokens device int32 [B]; `index` is the draw index
  * that keys the Philox stream (token position within a generation). Synchronises the stream. */
 int b2_op_sample(const float* logits, int B, int V, const b2_sampling* sampling, int index, int32_t* out_tokens, void* stream);
+/* b2_op_sample with logits processors: proc (nullable) [B], row b's history is proc[b]'s prompt ids (nothing generated yet).
+ * out_processed (nullable, device fp32 [B,V]) receives each row's logits after the processors and before temperature. */
+int b2_op_sample_ex(const float* logits, int B, int V, const b2_sampling* sampling, const b2_logits_proc* proc, int index,
+                    int32_t* out_tokens, float* out_processed, void* stream);
 
 #ifdef __cplusplus
 }

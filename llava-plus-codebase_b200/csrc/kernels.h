@@ -233,13 +233,39 @@ struct RowState {
     unsigned long long seed;
     int index;                // draws made for this request so far
 };
+// History-aware logits processing of one row (HF RepetitionPenalty -> NoRepeatNGram -> MinLength / MinNewTokens), applied by
+// sample_publish before selection. Device-resident like RowState, so a captured decode graph stays valid when it changes.
+constexpr int kProcMaxEos = 8;
+struct ProcRow {
+    int on;                   // 0: the row is selected from its raw logits and its history is not kept
+    float penalty;            // repetition penalty, 1 = off
+    int ngram;                // no_repeat_ngram_size, 0 = off
+    int min_gen;              // eos ids are banned while fewer than min_gen tokens were generated
+    int n_eos;
+    int eos[kProcMaxEos];
+    int prompt_len;           // history[0, prompt_len) is the caller's prompt row; what follows was generated
+    int hist_len;
+};
+// Per-cache processing state: rows[B], history int32 [B][cap] (cap = max_seq + 1), presence bitmap uint32 [B][words] of the
+// history's ids in [0, V). rows == nullptr: no row of this cache has ever had processors on.
+struct ProcState {
+    ProcRow* rows;
+    int32_t* hist;
+    uint32_t* bits;
+    int cap, words;
+};
 enum { SP_SELECT = 1,     // choose from `logits` (argmax or sample) and write tok[b]; otherwise tok[b] is already chosen
        SP_WRITE_OUT = 2,  // out_tokens[(*step_counter + step_offset) * B + b] = token
        SP_BUMP = 4 };     // last row: *step_counter += 1, cur_len[b] += 1
 int sample_state_set(SampleState* st_dev, const SampleState& v, cudaStream_t stream);
+// `proc` processes rows whose ProcRow is on (and appends the chosen token to their history); `processed_out` (nullable, fp32
+// [B,V]) receives each selected row's logits after processing and before temperature
 int sample_publish(const float* logits, int V, int B, SampleState* st_dev, RowState* rows_dev, int32_t* tok, int32_t* out_tokens,
                    int32_t* step_counter, int32_t* cur_len, int32_t* ring_dev, int ring_cap, int flags, int step_offset,
-                   cudaStream_t stream);
+                   const ProcState& proc, float* processed_out, cudaStream_t stream);
+// row := v, its history := ids[0, len) (int64, device) followed by `first_token` when >= 0, and its bitmap rebuilt from those ids
+int proc_seed(const ProcState& proc, int row, const ProcRow& v, const int64_t* ids, int len, int first_token, int V,
+              cudaStream_t stream);
 int row_state_set(RowState* row_dev, const RowState& v, int32_t* tok_dev, int token, cudaStream_t stream);
 
 // ---- beam search (beam.cu) ---------------------------------------------------------------------------------------------------

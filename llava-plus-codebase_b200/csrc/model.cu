@@ -182,6 +182,11 @@ struct b2_kv {
     // b2_beam_step (allocated by the first call): beam -> slot map and running scores [2][max_batch], the per-row candidate
     // keys of beam_topk, and its [B, K] outputs (scores, tokens, beams)
     DevBuf beam_in, beam_ws, beam_out;
+    // history-aware logits processing (b2_stream_begin_ex / b2_batch_set_row_ex; allocated by the first call that turns it on):
+    // ProcRow[max_batch], history int32 [max_batch][max_seq + 1], presence bitmap uint32 [max_batch][ceil(V / 32)]
+    DevBuf proc_rows, proc_hist, proc_bits;
+    std::vector<char> proc_on;  // host copy of ProcRow::on per slot
+    bool any_proc() const { for (char c : proc_on) if (c) return true; return false; }
     bool counted = false;  // included in m->kv_live
     bool e4m3() const { return dtype == B2_KV_E4M3; }
     size_t elem_bytes() const { return e4m3() ? 1 : 2; }
@@ -192,6 +197,14 @@ struct b2_kv {
 };
 
 namespace {
+
+ProcState proc_state(const b2_kv* kv) {
+    ProcState p = {};
+    if (kv->proc_rows.p == nullptr) return p;
+    p.rows = kv->proc_rows.as<ProcRow>(); p.hist = kv->proc_hist.as<int32_t>(); p.bits = kv->proc_bits.as<uint32_t>();
+    p.cap = kv->max_seq + 1; p.words = (kv->m->d.vocab + 31) / 32;
+    return p;
+}
 
 bool starts_with(const std::string& s, const char* p) { return s.rfind(p, 0) == 0; }
 
@@ -646,7 +659,7 @@ int decode_step_launch(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     // step / cache-length counters in one launch
     B2_TRY(sample_publish(m->logits.as<float>(), V, B, kv->sstate.as<SampleState>(), kv->rows_dev.as<RowState>(), kv->tok.as<int32_t>(),
                           kv->out_tokens.as<int32_t>(), kv->step_counter.as<int32_t>(), kv->len_dev.as<int32_t>(),
-                          kv->ring_dev, kv->ring_cap, SP_SELECT | SP_WRITE_OUT | SP_BUMP, 0, st));
+                          kv->ring_dev, kv->ring_cap, SP_SELECT | SP_WRITE_OUT | SP_BUMP, 0, proc_state(kv), nullptr, st));
     return 0;
 }
 
@@ -707,9 +720,9 @@ int decode_step_mega(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     kv->mega_bar_base += (unsigned int)(5 * d.layers + 2) * (unsigned int)num_sms();
     p.eps = d.rms_eps; p.theta = d.rope_theta;
     p.scale_log2 = (1.0f / sqrtf((float)m->hd)) * 1.4426950408889634f;
-    // greedy streaming: the kernel's fused argmax publishes to the host ring itself; with do_sample the sample_publish
-    // launch below overrides the fused argmax (token feedback, out_tokens slot) and publishes instead
-    const bool sampling = kv->samp_host.do_sample != 0 || kv->samp_host.per_row != 0;
+    // greedy streaming: the kernel's fused argmax publishes to the host ring itself; with do_sample (or logits processors) the
+    // sample_publish launch below overrides the fused argmax (token feedback, out_tokens slot) and publishes instead
+    const bool sampling = kv->samp_host.do_sample != 0 || kv->samp_host.per_row != 0 || kv->any_proc();
     if (!sampling && kv->samp_host.tag != 0) { p.sstate = kv->sstate.as<SampleState>(); p.ring = kv->ring_dev; p.ring_cap = kv->ring_cap; }
     if (kv->samp_host.per_row) p.rows = kv->rows_dev.as<RowState>();
     {   // tuning knobs, re-read every launch so a sweep can flip them inside one process (scripts/mega_sweep.py)
@@ -753,7 +766,7 @@ int decode_step_mega(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     if (sampling)
         B2_TRY(sample_publish(m->logits.as<float>(), d.vocab, B, kv->sstate.as<SampleState>(), kv->rows_dev.as<RowState>(), kv->tok.as<int32_t>(),
                               kv->out_tokens.as<int32_t>(), kv->step_counter.as<int32_t>(), kv->len_dev.as<int32_t>(),
-                              kv->ring_dev, kv->ring_cap, SP_SELECT | SP_WRITE_OUT, -1, st));
+                              kv->ring_dev, kv->ring_cap, SP_SELECT | SP_WRITE_OUT, -1, proc_state(kv), nullptr, st));
     return 0;
 }
 
@@ -821,7 +834,7 @@ int b2_init(int device) {
 }
 
 const char* b2_last_error(void) { return g_err; }
-int b2_version(void) { return 5; }
+int b2_version(void) { return 6; }
 unsigned long long b2_launch_count(void) { return g_launch_count; }
 
 int b2_model_create(const b2_model_desc* desc, b2_model** out) {
@@ -1279,7 +1292,7 @@ int b2_kv_destroy(b2_kv* kv) {
     if (kv->ev_join) cudaEventDestroy(kv->ev_join);
     DevBuf* bs[] = {&kv->k, &kv->v, &kv->kscale, &kv->vscale, &kv->len_dev, &kv->tok, &kv->step_counter, &kv->out_tokens, &kv->attn_partial,
                     &kv->attn_counters, &kv->mega_layers, &kv->mega_sync, &kv->sk_partial, &kv->sk_counters, &kv->sstate, &kv->rows_dev, &kv->rope_tab,
-                    &kv->beam_in, &kv->beam_ws, &kv->beam_out};
+                    &kv->beam_in, &kv->beam_ws, &kv->beam_out, &kv->proc_rows, &kv->proc_hist, &kv->proc_bits};
     for (DevBuf* b : bs) b->free();
     delete kv;
     return 0;
@@ -1530,11 +1543,77 @@ static int set_sampling(b2_kv* kv, const SampleState& v, bool force, cudaStream_
     kv->samp_valid = true;
     return 0;
 }
+// every slot selects from its raw logits again (a no-op on a cache whose processors are off)
+static int proc_all_off(b2_kv* kv, cudaStream_t st) {
+    if (!kv->any_proc()) return 0;
+    B2_CUDA_CHECK(cudaMemsetAsync(kv->proc_rows.p, 0, kv->proc_rows.bytes, st));
+    kv->proc_on.assign(kv->max_batch, 0);
+    return 0;
+}
 static int set_greedy_unpublished(b2_kv* kv, cudaStream_t st) {
     SampleState v = {};
     v.temperature = 1.f; v.top_p = 1.f;
     kv->stream_B = 0;  // any streaming generation on this cache is over
+    B2_TRY(proc_all_off(kv, st));
     return set_sampling(kv, v, false, st);
+}
+// b2_logits_proc -> ProcRow (on = 0 when every processor is at its off value); prompt ids are checked against `cap`
+static int proc_row_of(const b2_logits_proc* lp, int cap, ProcRow* out, const char* who) {
+    *out = ProcRow{};
+    out->penalty = 1.f;
+    if (lp == nullptr) return 0;
+    B2_CHECK_ARG(lp->repetition_penalty > 0.f && lp->repetition_penalty < INFINITY, "%s: repetition_penalty must be positive and finite (got %g)",
+                 who, (double)lp->repetition_penalty);
+    B2_CHECK_ARG(lp->no_repeat_ngram_size >= 0, "%s: no_repeat_ngram_size must be >= 0 (got %d)", who, lp->no_repeat_ngram_size);
+    B2_CHECK_ARG(lp->n_eos >= 0 && lp->n_eos <= kProcMaxEos, "%s: n_eos must be in [0, %d] (got %d)", who, kProcMaxEos, lp->n_eos);
+    B2_CHECK_ARG(lp->prompt_len >= 0 && (lp->prompt_len == 0 || lp->prompt_ids != nullptr), "%s: bad prompt ids", who);
+    out->penalty = lp->repetition_penalty;
+    out->ngram = lp->no_repeat_ngram_size;
+    out->n_eos = lp->n_eos;
+    for (int i = 0; i < lp->n_eos; ++i) out->eos[i] = lp->eos_ids[i];
+    out->min_gen = lp->n_eos > 0 && lp->min_generated > 0 ? lp->min_generated : 0;
+    out->on = (out->penalty != 1.f || out->ngram > 0 || out->min_gen > 0) ? 1 : 0;
+    out->prompt_len = lp->prompt_len;
+    out->hist_len = lp->prompt_len;
+    B2_CHECK_ARG(!out->on || lp->prompt_len + 1 <= cap, "%s: prompt of %d ids exceeds the history capacity %d", who, lp->prompt_len, cap);
+    return 0;
+}
+// the cache's processing state, allocated on first use; a decode graph captured before then does not read it and is dropped.
+// Every row starts off, zeroed on the caller's stream `st`: the seeding and the decode steps that read the state are ordered
+// after it there, which a memset on the legacy stream would not be when `st` is a non-blocking stream.
+static int proc_alloc(b2_kv* kv, cudaStream_t st) {
+    if (kv->proc_rows.p != nullptr) return 0;
+    const size_t words = (size_t)(kv->m->d.vocab + 31) / 32;
+    int r = kv->proc_rows.alloc((size_t)kv->max_batch * sizeof(ProcRow));
+    if (r == 0) r = kv->proc_hist.alloc((size_t)kv->max_batch * (kv->max_seq + 1) * sizeof(int32_t));
+    if (r == 0) r = kv->proc_bits.alloc((size_t)kv->max_batch * words * sizeof(uint32_t));
+    if (r == 0 && cudaMemsetAsync(kv->proc_rows.p, 0, kv->proc_rows.bytes, st) != cudaSuccess) {
+        set_error("proc_alloc: %s", cudaGetErrorString(cudaGetLastError()));
+        r = -2;
+    }
+    if (r != 0) {  // all or nothing: proc_rows != nullptr means the whole state exists
+        kv->proc_rows.free(); kv->proc_hist.free(); kv->proc_bits.free();
+        return r;
+    }
+    kv->proc_on.assign(kv->max_batch, 0);
+    if (kv->graph) { cudaGraphExecDestroy(kv->graph); kv->graph = nullptr; kv->graph_B = 0; }
+    return 0;
+}
+// slot `row` := v; its history seeded from the prompt ids (and first_token when >= 0) when v is on
+static int proc_set_row(b2_kv* kv, int row, const ProcRow& v, const int64_t* ids, int first_token, cudaStream_t st) {
+    if (!v.on) {
+        if (kv->proc_rows.p != nullptr && kv->proc_on[row]) {
+            B2_CUDA_CHECK(cudaMemsetAsync(kv->proc_rows.as<ProcRow>() + row, 0, sizeof(ProcRow), st));
+            kv->proc_on[row] = 0;
+        }
+        return 0;
+    }
+    B2_TRY(proc_alloc(kv, st));
+    ProcRow r = v;
+    if (first_token >= 0) r.hist_len += 1;
+    B2_TRY(proc_seed(proc_state(kv), row, r, ids, v.prompt_len, first_token, kv->m->d.vocab, st));
+    kv->proc_on[row] = 1;
+    return 0;
 }
 static bool is_device_pointer(const void* p) {
     cudaPointerAttributes attr;
@@ -1713,6 +1792,11 @@ int b2_beam_step(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, void* strea
 
 // ---- streaming decode: the device runs ahead, the host reads tokens from mapped pinned memory ---------------------------
 int b2_stream_begin(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sp, void* stream) {
+    return b2_stream_begin_ex(m, kv, logits, B, sp, nullptr, stream);
+}
+
+int b2_stream_begin_ex(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sp, const b2_logits_proc* proc,
+                       void* stream) {
     B2_CHECK_ARG(m && kv && logits && kv->m == m, "b2_stream_begin: bad handle");
     B2_CHECK_ARG(m->finalized, "b2_stream_begin: model not finalized");
     B2_CHECK_ARG(B >= 1 && B <= kv->max_batch, "b2_stream_begin: B=%d exceeds cache batch %d", B, kv->max_batch);
@@ -1729,14 +1813,20 @@ int b2_stream_begin(b2_model* m, b2_kv* kv, const float* logits, int B, const b2
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     for (int b = 0; b < B; ++b)
         B2_CHECK_ARG(kv->len_host[b] >= 1, "b2_stream_begin: sample %d has an empty cache (prefill first)", b);
+    std::vector<ProcRow> pr(B);
+    for (int b = 0; b < B; ++b) B2_TRY(proc_row_of(proc ? proc + b : nullptr, kv->max_seq + 1, &pr[b], "b2_stream_begin_ex"));
     kv->epoch += 1;
     v.tag = 1 + kv->epoch % 2047;
     B2_TRY(ws_enter(m, st));
     B2_TRY(set_sampling(kv, v, true, st));
     B2_CUDA_CHECK(cudaMemsetAsync(kv->step_counter.p, 0, 4, st));
-    // token 0: chosen from the prefill's last-position logits, published as ring entry 0, fed to the first decode step
+    B2_TRY(proc_all_off(kv, st));
+    for (int b = 0; b < B; ++b) B2_TRY(proc_set_row(kv, b, pr[b], proc ? proc[b].prompt_ids : nullptr, -1, st));
+    // token 0: chosen from the prefill's last-position logits (processed over the prompt history), published as ring entry 0,
+    // fed to the first decode step
     B2_TRY(sample_publish(logits, m->d.vocab, B, kv->sstate.as<SampleState>(), kv->rows_dev.as<RowState>(), kv->tok.as<int32_t>(), nullptr,
-                          kv->step_counter.as<int32_t>(), kv->len_dev.as<int32_t>(), kv->ring_dev, kv->ring_cap, SP_SELECT, 0, st));
+                          kv->step_counter.as<int32_t>(), kv->len_dev.as<int32_t>(), kv->ring_dev, kv->ring_cap, SP_SELECT, 0,
+                          proc_state(kv), nullptr, st));
     kv->stream_B = B; kv->stream_tag = v.tag; kv->stream_scheduled = 1;
     return ws_leave(m, st);
 }
@@ -1779,6 +1869,7 @@ int b2_batch_begin(b2_model* m, b2_kv* kv, int B, void* stream) {
     B2_TRY(ws_enter(m, st));
     B2_TRY(set_sampling(kv, v, true, st));
     B2_CUDA_CHECK(cudaMemsetAsync(kv->step_counter.p, 0, 4, st));
+    B2_TRY(proc_all_off(kv, st));
     B2_CUDA_CHECK(cudaMemsetAsync(kv->rows_dev.p, 0, (size_t)kv->max_batch * sizeof(RowState), st));
     B2_CUDA_CHECK(cudaMemsetAsync(kv->len_dev.p, 0, (size_t)kv->max_batch * 4, st));
     B2_CUDA_CHECK(cudaMemsetAsync(kv->tok.p, 0, (size_t)kv->max_batch * 4, st));
@@ -1789,6 +1880,11 @@ int b2_batch_begin(b2_model* m, b2_kv* kv, int B, void* stream) {
 }
 
 int b2_batch_set_row(b2_model* m, b2_kv* kv, int slot, int active, const b2_sampling* sp, int first_token, void* stream) {
+    return b2_batch_set_row_ex(m, kv, slot, active, sp, nullptr, first_token, stream);
+}
+
+int b2_batch_set_row_ex(b2_model* m, b2_kv* kv, int slot, int active, const b2_sampling* sp, const b2_logits_proc* proc,
+                        int first_token, void* stream) {
     B2_CHECK_ARG(m && kv && kv->m == m && slot >= 0 && slot < kv->stream_B, "b2_batch_set_row: bad slot %d", slot);
     B2_CHECK_ARG(kv->samp_host.per_row != 0, "b2_batch_set_row: b2_batch_begin first");
     RowState v = {};
@@ -1797,11 +1893,15 @@ int b2_batch_set_row(b2_model* m, b2_kv* kv, int slot, int active, const b2_samp
         B2_CHECK_ARG(sp->temperature > 0.f && sp->top_p > 0.f && sp->top_p <= 1.f && sp->top_k >= 0, "b2_batch_set_row: bad sampling parameters");
         v.do_sample = 1; v.temperature = sp->temperature; v.top_p = sp->top_p; v.top_k = sp->top_k; v.seed = sp->seed;
     }
+    ProcRow pr;
+    B2_TRY(proc_row_of(active ? proc : nullptr, kv->max_seq + 1, &pr, "b2_batch_set_row_ex"));
+    B2_CHECK_ARG(!pr.on || (first_token >= 0 && first_token < m->d.vocab), "b2_batch_set_row_ex: first_token %d out of range", first_token);
     std::lock_guard<std::mutex> lk(m->mu);
     DeviceGuard dg(m->device);
     B2_CHECK_ARG(!active || kv->len_host[slot] >= 1, "b2_batch_set_row: slot %d has an empty cache (prefill it first)", slot);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     B2_TRY(ws_enter(m, st));
+    B2_TRY(proc_set_row(kv, slot, pr, proc ? proc->prompt_ids : nullptr, first_token, st));  // history: prompt, then first_token
     B2_TRY(row_state_set(kv->rows_dev.as<RowState>() + slot, v, active ? kv->tok.as<int32_t>() + slot : nullptr, first_token, st));
     if (!active) {  // a freed slot restarts from an empty cache
         B2_CUDA_CHECK(cudaMemsetAsync(kv->len_dev.as<int32_t>() + slot, 0, 4, st));
@@ -1858,6 +1958,11 @@ int b2_op_preprocess_clip(const b2_preprocess_plan* pl, void* stream) {
 
 // standalone selection (unit tests, first-token choice outside a streaming generation): out_tokens[b] (device int32)
 int b2_op_sample(const float* logits, int B, int V, const b2_sampling* sp, int index, int32_t* out_tokens, void* stream) {
+    return b2_op_sample_ex(logits, B, V, sp, nullptr, index, out_tokens, nullptr, stream);
+}
+
+int b2_op_sample_ex(const float* logits, int B, int V, const b2_sampling* sp, const b2_logits_proc* proc, int index, int32_t* out_tokens,
+                    float* out_processed, void* stream) {
     B2_CHECK_ARG(logits && out_tokens && B >= 1 && V >= 1 && index >= 0, "b2_op_sample: bad argument");
     SampleState v = {};
     v.temperature = 1.f; v.top_p = 1.f;
@@ -1866,12 +1971,40 @@ int b2_op_sample(const float* logits, int B, int V, const b2_sampling* sp, int i
         v.do_sample = 1; v.temperature = sp->temperature; v.top_p = sp->top_p; v.top_k = sp->top_k; v.seed = sp->seed;
     }
     v.pub_counter = index;
+    // processors: a scratch state whose row b holds proc[b]'s prompt ids as its history
+    std::vector<ProcRow> pr(proc ? B : 0);
+    int cap = 1;
+    bool any = false;
+    for (int b = 0; b < (int)pr.size(); ++b) {
+        B2_TRY(proc_row_of(proc + b, INT_MAX, &pr[b], "b2_op_sample_ex"));
+        cap = std::max(cap, proc[b].prompt_len + 1);
+        any = any || pr[b].on;
+    }
+    // one scratch buffer: SampleState, then (with processors) ProcRow[B], history int32 [B][cap] and the bitmap [B][words]
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const int words = (V + 31) / 32;
+    static_assert(sizeof(SampleState) <= 256, "b2_op_sample_ex scratch layout");
+    const size_t off_rows = 256, off_hist = off_rows + (size_t)B * sizeof(ProcRow), off_bits = off_hist + (size_t)B * cap * sizeof(int32_t);
     DevBuf tmp;
-    B2_TRY(tmp.alloc(sizeof(SampleState) + 64));
-    int r = sample_state_set(tmp.as<SampleState>(), v, st);
+    B2_TRY(tmp.alloc(any ? off_bits + (size_t)B * words * sizeof(uint32_t) : sizeof(SampleState) + 64));
+    ProcState ps = {};
+    int r = 0;
+    if (any) {
+        ps.rows = reinterpret_cast<ProcRow*>(tmp.as<char>() + off_rows);
+        ps.hist = reinterpret_cast<int32_t*>(tmp.as<char>() + off_hist);
+        ps.bits = reinterpret_cast<uint32_t*>(tmp.as<char>() + off_bits);
+        ps.cap = cap; ps.words = words;
+        if (cudaMemsetAsync(ps.rows, 0, (size_t)B * sizeof(ProcRow), st) != cudaSuccess) {
+            set_error("b2_op_sample_ex: %s", cudaGetErrorString(cudaGetLastError()));
+            r = -2;
+        }
+        for (int b = 0; b < B && r == 0; ++b)
+            if (pr[b].on) r = proc_seed(ps, b, pr[b], proc[b].prompt_ids, pr[b].prompt_len, -1, V, st);
+    }
+    if (r == 0) r = sample_state_set(tmp.as<SampleState>(), v, st);
     if (r == 0)
-        r = sample_publish(logits, V, B, tmp.as<SampleState>(), nullptr, out_tokens, nullptr, nullptr, nullptr, nullptr, 0, SP_SELECT, 0, st);
+        r = sample_publish(logits, V, B, tmp.as<SampleState>(), nullptr, out_tokens, nullptr, nullptr, nullptr, nullptr, 0, SP_SELECT, 0,
+                           ps, out_processed, st);
     cudaError_t e = cudaStreamSynchronize(st);
     tmp.free();
     if (r != 0) return r;

@@ -139,10 +139,42 @@ __device__ __forceinline__ uint32_t radix_select(const float* s_x, int V, unsign
     return *s_prefix;
 }
 
+// HF's history-aware processors over the staged row s_x, in transformers' order (repetition -> no-repeat-ngram -> min_length /
+// min_new_tokens). Ids of the history outside [0, V) (IMAGE_TOKEN_INDEX placeholders) are never penalised or banned.
+__device__ __forceinline__ void process_row(float* s_x, int V, const ProcState& proc, int b, int tid) {
+    const ProcRow& pr = proc.rows[b];
+    const int L = pr.hist_len, n = pr.ngram;
+    const float p = pr.penalty;
+    const int32_t* hist = proc.hist + (size_t)b * proc.cap;
+    const uint32_t* bits = proc.bits + (size_t)b * proc.words;
+    __syncthreads();  // the staged row is complete
+    if (p != 1.0f) {  // RepetitionPenaltyLogitsProcessor: once per distinct id of the history, IEEE fp32
+        for (int i = tid; i < V; i += SP_THREADS)
+            if ((bits[i >> 5] >> (i & 31)) & 1u) {
+                const float x = s_x[i];
+                s_x[i] = x < 0.f ? __fmul_rn(x, p) : __fdiv_rn(x, p);
+            }
+        __syncthreads();
+    }
+    if (n > 0 && L + 1 >= n) {  // NoRepeatNGramLogitsProcessor: every n-gram whose first n-1 ids equal the last n-1 ids
+        const int32_t* tail = hist + (L - n + 1);
+        for (int s = tid; s <= L - n; s += SP_THREADS) {
+            bool match = true;
+            for (int j = 0; j < n - 1 && match; ++j) match = hist[s + j] == tail[j];
+            const int t = hist[s + n - 1];
+            if (match && t >= 0 && t < V) s_x[t] = -INFINITY;  // idempotent: threads may ban the same id
+        }
+    }
+    if (L - pr.prompt_len < pr.min_gen && tid < pr.n_eos) {  // MinLength / MinNewTokensLength
+        const int e = pr.eos[tid];
+        if (e >= 0 && e < V) s_x[e] = -INFINITY;
+    }
+}
+
 __global__ void __launch_bounds__(SP_THREADS, 1)
 sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleState* st, RowState* rows, int32_t* tok, int32_t* out_tokens,
                       int32_t* step_counter, int32_t* cur_len, volatile int32_t* ring, int ring_cap, int flags,
-                      int step_offset) {
+                      int step_offset, ProcState proc, float* processed_out) {
     extern __shared__ __align__(16) uint8_t sp_smem[];
     float* s_x = reinterpret_cast<float*>(sp_smem);
     __shared__ unsigned long long s_hist[256];
@@ -165,18 +197,29 @@ sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleStat
     const unsigned long long seed = per_row ? rows[b].seed : st->seed;
     const int pub = st->pub_counter;
     const int draw = per_row ? rows[b].index : pub;
+    const bool select = active && (flags & SP_SELECT);
+    const bool proc_on = proc.rows != nullptr && proc.rows[b].on != 0 && active;
     int choice = 0;
+    const float* row = logits + (size_t)b * V;
+    if (select && (proc_on || processed_out != nullptr)) {
+        // stage the row and run the processors in HF's order over it; selection below reads the staged row
+        for (int i = tid; i < V; i += SP_THREADS) s_x[i] = row[i];
+        if (proc_on) process_row(s_x, V, proc, b, tid);
+        __syncthreads();
+        if (processed_out != nullptr)
+            for (int i = tid; i < V; i += SP_THREADS) processed_out[(size_t)b * V + i] = s_x[i];
+        row = s_x;
+    }
 
     if (!active) {
         choice = tok[b];  // an idle slot keeps its token; nothing is selected or counted for it
     } else if (!(flags & SP_SELECT)) {
         choice = tok[b];  // already chosen by the producer of `tok` (decode megakernel's fused argmax)
     } else if (!do_sample) {
-        choice = block_argmax(logits + (size_t)b * V, V, tid, s_v, s_i, nullptr);
+        choice = block_argmax(row, V, tid, s_v, s_i, nullptr);
     } else {
-        const float* row = logits + (size_t)b * V;
         const float inv_t = 1.0f / temperature;
-        for (int i = tid; i < V; i += SP_THREADS) s_x[i] = row[i] * inv_t;
+        for (int i = tid; i < V; i += SP_THREADS) s_x[i] = row[i] * inv_t;  // in place when staged: each thread its own i
         __syncthreads();
         // ---- top-k: keep everything >= the k-th largest scaled logit (ties kept, like TopKLogitsWarper) ----
         const int k = top_k;
@@ -251,6 +294,15 @@ sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleStat
     if (tid == 0) {
         if ((flags & SP_SELECT) && active) tok[b] = choice;
         if (per_row && active) rows[b].index = draw + 1;
+        if (proc_on) {  // the chosen token joins the row's history
+            ProcRow& pr = proc.rows[b];
+            const int n = pr.hist_len;
+            if (n < proc.cap) {
+                proc.hist[(size_t)b * proc.cap + n] = choice;
+                pr.hist_len = n + 1;
+            }
+            if (choice >= 0 && choice < V) proc.bits[(size_t)b * proc.words + (choice >> 5)] |= 1u << (choice & 31);
+        }
         if (flags & SP_WRITE_OUT) out_tokens[(size_t)(*step_counter + step_offset) * B + b] = choice;
         if (ring != nullptr && st->tag != 0) {
             // the tag advances every time the ring wraps, so an entry left from ring_cap steps ago is never taken for a new one
@@ -269,6 +321,22 @@ sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleStat
             }
         }
     }
+}
+
+__global__ void __launch_bounds__(SP_THREADS, 1)
+proc_seed_kernel(ProcState proc, int row, ProcRow v, const int64_t* __restrict__ ids, int len, int first_token, int V) {
+    uint32_t* bits = proc.bits + (size_t)row * proc.words;
+    int32_t* hist = proc.hist + (size_t)row * proc.cap;
+    const int tid = threadIdx.x;
+    for (int i = tid; i < proc.words; i += SP_THREADS) bits[i] = 0u;
+    __syncthreads();
+    for (int i = tid; i <= len; i += SP_THREADS) {
+        const long long id = i < len ? ids[i] : (long long)first_token;
+        if (i == len && first_token < 0) break;
+        hist[i] = (int32_t)id;
+        if (id >= 0 && id < V) atomicOr(&bits[id >> 5], 1u << (id & 31));
+    }
+    if (tid == 0) proc.rows[row] = v;
 }
 
 __global__ void sample_state_set_kernel(SampleState* st, SampleState v) {
@@ -297,9 +365,18 @@ int row_state_set(RowState* row_dev, const RowState& v, int32_t* tok_dev, int to
     return 0;
 }
 
+int proc_seed(const ProcState& proc, int row, const ProcRow& v, const int64_t* ids, int len, int first_token, int V,
+              cudaStream_t stream) {
+    B2_CHECK_ARG(proc.rows != nullptr && len >= 0 && (len == 0 || ids != nullptr), "proc_seed: bad argument");
+    B2_CHECK_ARG(len + (first_token >= 0 ? 1 : 0) <= proc.cap, "proc_seed: history of %d ids exceeds its capacity %d", len, proc.cap);
+    proc_seed_kernel<<<1, SP_THREADS, 0, stream>>>(proc, row, v, ids, len, first_token, V);
+    B2_LAUNCH_CHECK();
+    return 0;
+}
+
 int sample_publish(const float* logits, int V, int B, SampleState* st_dev, RowState* rows_dev, int32_t* tok, int32_t* out_tokens,
                    int32_t* step_counter, int32_t* cur_len, int32_t* ring_dev, int ring_cap, int flags, int step_offset,
-                   cudaStream_t stream) {
+                   const ProcState& proc, float* processed_out, cudaStream_t stream) {
     B2_CHECK_ARG(B >= 1 && V >= 1 && st_dev != nullptr && tok != nullptr, "sample_publish: bad argument");
     B2_CHECK_ARG(V < (1 << 20), "sample_publish: vocab %d does not fit the 20-bit token field of the host ring", V);
     const size_t smem = sample_smem_bytes(V);
@@ -310,7 +387,7 @@ int sample_publish(const float* logits, int V, int B, SampleState* st_dev, RowSt
         attr = smem;
     }
     B2_CUDA_CHECK(launch_pdl(sample_publish_kernel, dim3(B), dim3(SP_THREADS), smem, stream, logits, V, B, st_dev, rows_dev, tok,
-                             out_tokens, step_counter, cur_len, ring_dev, ring_cap, flags, step_offset));
+                             out_tokens, step_counter, cur_len, ring_dev, ring_cap, flags, step_offset, proc, processed_out));
     B2_LAUNCH_CHECK();
     return 0;
 }

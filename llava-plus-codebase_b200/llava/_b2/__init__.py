@@ -62,6 +62,49 @@ class BeamStepArgs(_c.Structure):
                 ("beam_scores_host", _vp), ("out_scores_host", _vp), ("out_tokens_host", _vp), ("out_beams_host", _vp)]
 
 
+class LogitsProc(_c.Structure):
+    """b2_logits_proc (include/b2llava.h): history-aware logits processors of one row; `prompt_ids` is a device int64 pointer."""
+    _fields_ = [("repetition_penalty", _c.c_float), ("no_repeat_ngram_size", _c.c_int32), ("min_generated", _c.c_int32),
+                ("n_eos", _c.c_int32), ("eos_ids", _c.c_int32 * 8), ("prompt_ids", _vp), ("prompt_len", _c.c_int32)]
+
+
+MAX_PROC_EOS = 8
+
+
+def make_logits_proc(prompt_row, repetition_penalty=1.0, no_repeat_ngram_size=0, min_generated=0, eos_ids=()):
+    """LogitsProc over `prompt_row` (device int64 [L], kept alive as `.ids` of the result; a caller that hands the struct to
+    work on another stream records that stream on it), or None when every processor is at its off value. min_generated: eos ids are banned while fewer tokens were generated."""
+    eos = sorted(set(int(e) for e in eos_ids))
+    if len(eos) > MAX_PROC_EOS:
+        raise ValueError(f"at most {MAX_PROC_EOS} eos ids are supported with logits processors, got {len(eos)}")
+    p = float(1.0 if repetition_penalty is None else repetition_penalty)
+    n = int(no_repeat_ngram_size or 0)
+    mg = int(min_generated or 0) if eos else 0
+    if p == 1.0 and n == 0 and mg <= 0:
+        return None
+    if prompt_row.dtype != torch.int64 or prompt_row.dim() != 1 or not prompt_row.is_cuda or not prompt_row.is_contiguous():
+        raise ValueError("prompt_row must be a contiguous 1-D int64 CUDA tensor")
+    lp = LogitsProc(p, n, max(mg, 0), len(eos))
+    for i, e in enumerate(eos):
+        lp.eos_ids[i] = e
+    lp.prompt_ids = prompt_row.data_ptr() if prompt_row.numel() else None
+    lp.prompt_len = int(prompt_row.numel())
+    lp.ids = prompt_row  # the tensor behind prompt_ids: whoever holds the struct keeps the ids alive
+    return lp
+
+
+def _proc_array(procs, B):
+    """ctypes array of B LogitsProc (None entries = off), or None when every row is off."""
+    if procs is None or all(p is None for p in procs):
+        return None
+    if len(procs) != B:
+        raise ValueError(f"{len(procs)} logits processors for {B} rows")
+    arr = (LogitsProc * B)()
+    for b, p in enumerate(procs):
+        arr[b] = p if p is not None else LogitsProc(1.0, 0, 0, 0)
+    return arr
+
+
 def make_sampling(do_sample=False, temperature=1.0, top_p=1.0, top_k=0, seed=0):
     return Sampling(int(bool(do_sample)), float(temperature), float(1.0 if top_p is None else top_p),
                     int(top_k or 0), int(seed) & (2**64 - 1))
@@ -94,15 +137,18 @@ SIGNATURES = {
     "b2_splice_ids": (_i32, [_vp, _vp, _i32, _i32, _i32, _c.POINTER(_c.c_int32), _i32, _vp, _i32, _vp, _vp]),
     "b2_async_error": (_i32, [_vp, _c.POINTER(_c.c_int)]),
     "b2_stream_begin": (_i32, [_vp, _vp, _vp, _i32, _c.POINTER(Sampling), _vp]),
+    "b2_stream_begin_ex": (_i32, [_vp, _vp, _vp, _i32, _c.POINTER(Sampling), _c.POINTER(LogitsProc), _vp]),
     "b2_stream_enqueue": (_i32, [_vp, _vp, _i32, _vp]),
     "b2_stream_wait": (_i32, [_vp, _i32, _c.POINTER(_c.c_int32), _i32]),
     "b2_op_preprocess_clip": (_i32, [_c.POINTER(PreprocessPlan), _vp]),
     "b2_op_sample": (_i32, [_vp, _i32, _i32, _c.POINTER(Sampling), _i32, _vp, _vp]),
+    "b2_op_sample_ex": (_i32, [_vp, _i32, _i32, _c.POINTER(Sampling), _c.POINTER(LogitsProc), _i32, _vp, _vp, _vp]),
     "b2_prefill": (_i32, [_vp, _vp, _vp, _c.POINTER(_c.c_int32), _i32, _i32, _vp, _i32, _vp]),
     "b2_prefill_slots": (_i32, [_vp, _vp, _vp, _c.POINTER(_c.c_int32), _i32, _i32, _i32, _vp, _i32, _vp]),
     "b2_prefill_at": (_i32, [_vp, _vp, _vp, _c.POINTER(_c.c_int32), _c.POINTER(_c.c_int32), _i32, _i32, _i32, _vp, _i32, _vp]),
     "b2_batch_begin": (_i32, [_vp, _vp, _i32, _vp]),
     "b2_batch_set_row": (_i32, [_vp, _vp, _i32, _i32, _c.POINTER(Sampling), _i32, _vp]),
+    "b2_batch_set_row_ex": (_i32, [_vp, _vp, _i32, _i32, _c.POINTER(Sampling), _c.POINTER(LogitsProc), _i32, _vp]),
     "b2_decode_step": (_i32, [_vp, _vp, _vp, _i32, _vp, _vp, _vp]),
     "b2_decode_greedy": (_i32, [_vp, _vp, _vp, _i32, _i32, _vp, _vp]),
     "b2_argmax": (_i32, [_vp, _i32, _i32, _vp, _vp]),
@@ -422,23 +468,34 @@ class Engine:
         return out
 
     # -- streaming decode (device runs ahead, host reads tokens from mapped pinned memory) ---------------
-    def stream_begin(self, kv, logits, sampling=None):
-        """Token 0 is chosen from the prefill logits [B, vocab] on the device and published as ring index 0."""
+    def stream_begin(self, kv, logits, sampling=None, procs=None):
+        """Token 0 is chosen from the prefill logits [B, vocab] on the device and published as ring index 0. `procs`: one
+        LogitsProc (or None) per row; rows with processors keep their history on the device for the whole generation."""
         logits = logits.contiguous()
         sp = sampling if sampling is not None else make_sampling()
+        B = int(logits.shape[0])
+        arr = _proc_array(procs, B)
         with torch.cuda.device(self.index):
-            check(self.lib.b2_stream_begin(self.handle, kv.handle, ptr(logits), int(logits.shape[0]), ctypes.byref(sp),
-                                           stream_ptr()), "b2_stream_begin")
+            if arr is None:
+                check(self.lib.b2_stream_begin(self.handle, kv.handle, ptr(logits), B, ctypes.byref(sp), stream_ptr()),
+                      "b2_stream_begin")
+            else:
+                check(self.lib.b2_stream_begin_ex(self.handle, kv.handle, ptr(logits), B, ctypes.byref(sp), arr, stream_ptr()),
+                      "b2_stream_begin_ex")
 
     def batch_begin(self, kv, B):
         with torch.cuda.device(self.index):
             check(self.lib.b2_batch_begin(self.handle, kv.handle, int(B), stream_ptr()), "b2_batch_begin")
 
-    def batch_set_row(self, kv, slot, active, sampling=None, first_token=0):
+    def batch_set_row(self, kv, slot, active, sampling=None, first_token=0, proc=None):
         sp = sampling if sampling is not None else make_sampling()
         with torch.cuda.device(self.index):
-            check(self.lib.b2_batch_set_row(self.handle, kv.handle, int(slot), int(bool(active)), ctypes.byref(sp), int(first_token),
-                                            stream_ptr()), "b2_batch_set_row")
+            if proc is None:
+                check(self.lib.b2_batch_set_row(self.handle, kv.handle, int(slot), int(bool(active)), ctypes.byref(sp),
+                                                int(first_token), stream_ptr()), "b2_batch_set_row")
+            else:
+                check(self.lib.b2_batch_set_row_ex(self.handle, kv.handle, int(slot), int(bool(active)), ctypes.byref(sp),
+                                                   ctypes.byref(proc), int(first_token), stream_ptr()), "b2_batch_set_row_ex")
 
     def stream_enqueue(self, kv, n_steps):
         with torch.cuda.device(self.index):
@@ -450,15 +507,23 @@ class Engine:
         check(self.lib.b2_stream_wait(kv.handle, int(index), out, int(timeout_ms)), "b2_stream_wait")
         return list(out)
 
-    def sample(self, logits, sampling, index=0):
-        """One selection per row of fp32 logits [B, V] with csrc/sampling.cu (greedy or temperature/top-k/top-p)."""
+    def sample(self, logits, sampling, index=0, procs=None, want_processed=False):
+        """One selection per row of fp32 logits [B, V] with csrc/sampling.cu (greedy or temperature/top-k/top-p). `procs`: one
+        LogitsProc (or None) per row, applied over its prompt history first. With want_processed, returns (tokens, the
+        processed logits [B, V] before temperature)."""
         logits = logits.to(device=self.device, dtype=torch.float32).contiguous()
         B, V = logits.shape
         out = torch.empty(B, dtype=torch.int32, device=self.device)
+        arr = _proc_array(procs, B)
+        processed = torch.empty(B, V, dtype=torch.float32, device=self.device) if want_processed else None
         with torch.cuda.device(self.index):
-            check(self.lib.b2_op_sample(ptr(logits), B, V, ctypes.byref(sampling), int(index), ptr(out), stream_ptr()),
-                  "b2_op_sample")
-        return out
+            if arr is None and processed is None:
+                check(self.lib.b2_op_sample(ptr(logits), B, V, ctypes.byref(sampling), int(index), ptr(out), stream_ptr()),
+                      "b2_op_sample")
+            else:
+                check(self.lib.b2_op_sample_ex(ptr(logits), B, V, ctypes.byref(sampling), arr, int(index), ptr(out),
+                                               None if processed is None else ptr(processed), stream_ptr()), "b2_op_sample_ex")
+        return (out, processed) if want_processed else out
 
     # -- beam search (generate(num_beams > 1); host half in llava/_b2/beam.py) ------------------------------------------------
     def kv_copy_slots(self, kv, src, dst, row_begin=0):

@@ -26,8 +26,9 @@ from . import LOGITS_LAST, make_sampling
 class Request:
     """One generation in flight. The consumer thread reads tokens with `get()`; `cancel()` retires it early."""
 
-    def __init__(self, embeds, length, sampling, max_new_tokens):
+    def __init__(self, embeds, length, sampling, max_new_tokens, proc=None):
         self.embeds, self.length, self.sampling, self.max_new_tokens = embeds, int(length), sampling, int(max_new_tokens)
+        self.proc = proc  # LogitsProc over the request's prompt ids (device), or None
         self.tokens = queue.Queue()
         self.produced = 0
         self.cancelled = False
@@ -82,15 +83,16 @@ class ContinuousBatcher:
         self.thread.start()
 
     # ---- consumer side -------------------------------------------------------------------------------------
-    def submit(self, embeds, length, sampling=None, max_new_tokens=20):
-        """embeds: bf16 [1, S, hidden] on the device (already spliced by the caller's thread); returns a Request."""
+    def submit(self, embeds, length, sampling=None, max_new_tokens=20, proc=None):
+        """embeds: bf16 [1, S, hidden] on the device (already spliced by the caller's thread); proc: the request's LogitsProc
+        (its prompt ids produced on the caller's stream, like embeds) or None; returns a Request."""
         if self.closed:
             raise RuntimeError("batcher is closed")
         if length + max_new_tokens > self.max_seq:
             raise ValueError(f"sequence {length} + {max_new_tokens} new tokens exceeds the batcher's cache ({self.max_seq})")
         ready = self._cuda.Event()
         ready.record()                          # the caller's stream produced `embeds`: the scheduler's stream waits for it
-        req = Request(embeds, length, sampling or make_sampling(), max_new_tokens)
+        req = Request(embeds, length, sampling or make_sampling(), max_new_tokens, proc)
         req.ready = ready
         self.pending.put(req)
         self.wake.set()
@@ -108,9 +110,16 @@ class ContinuousBatcher:
         req.slot = slot
         self.stream.wait_event(req.ready)
         logits = eng.prefill(self.kv, req.embeds, [req.length], LOGITS_LAST, slot0=slot)
-        first = int(eng.sample(logits, req.sampling, index=0).cpu()[0])      # admission is a sync point anyway
-        eng.check_async_error()
-        eng.batch_set_row(self.kv, slot, True, req.sampling, first)
+        if req.proc is None:
+            first = int(eng.sample(logits, req.sampling, index=0).cpu()[0])      # admission is a sync point anyway
+            eng.check_async_error()
+            eng.batch_set_row(self.kv, slot, True, req.sampling, first)
+        else:  # the first token is chosen over the prompt history; the slot's history is the prompt and that token
+            # the ids were made on the caller's stream and are read on this one, possibly after the caller dropped them
+            req.proc.ids.record_stream(self.stream)
+            first = int(eng.sample(logits, req.sampling, index=0, procs=[req.proc]).cpu()[0])
+            eng.check_async_error()
+            eng.batch_set_row(self.kv, slot, True, req.sampling, first, proc=req.proc)
         req.embeds = None
         self.active[slot] = req
         self.stats["admitted"] += 1

@@ -25,7 +25,8 @@ from transformers.modeling_outputs import CausalLMOutputWithPast
 
 from ..llava_arch import LlavaMetaModel, LlavaMetaForCausalLM
 from ..multimodal_encoder.clip_encoder import _Holder, _read_checkpoint_dir
-from ..._b2 import Engine, KVCache, LOGITS_ALL, LOGITS_LAST, ERR_SPLICE_SLOTS, INT32_MIN, kv_dtype_code, last_error, make_sampling
+from ..._b2 import (Engine, KVCache, LOGITS_ALL, LOGITS_LAST, ERR_SPLICE_SLOTS, INT32_MIN, kv_dtype_code, last_error, make_logits_proc,
+                    make_sampling)
 from ..._b2 import prefix as _prefix
 from ...constants import IMAGE_TOKEN_INDEX
 from ..llava_arch import build_source_index
@@ -479,6 +480,8 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         "prefix_allowed_tokens_fn": None, "constraints": None, "suppress_tokens": None, "begin_suppress_tokens": None,
         "forced_bos_token_id": None, "forced_eos_token_id": None, "assistant_model": None, "min_p": None,
     }
+    # implemented by the device's logits processing when config.b2_logits_processors / B2_LOGITS_PROCESSORS=1 opts in
+    _LOGITS_PROCESSOR_ARGS = ("repetition_penalty", "no_repeat_ngram_size", "min_new_tokens", "min_length")
     # accepted and without effect on this path
     _IGNORED_GENERATION_ARGS = {"synced_gpus", "early_stopping", "output_attentions", "output_hidden_states",
                                 "generation_config", "position_ids", "past_key_values", "renormalize_logits", "max_time"}
@@ -500,8 +503,12 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             inputs = input_ids
         if inputs is None:
             raise ValueError("generate() needs input ids")
+        proc_args = self._logits_processor_arguments(kwargs)
         beam_args = {}
         if num_beams != 1:
+            if proc_args:
+                raise NotImplementedError("logits processors (repetition_penalty, no_repeat_ngram_size, min_new_tokens, "
+                                          "min_length) together with num_beams > 1 are not implemented on the H100 path")
             if self._beam_search_cap() < 2:
                 raise NotImplementedError("beam search is not used on the LLaVA path (num_beams=1 everywhere)")
             beam_args = self._beam_arguments(num_beams, do_sample, temperature, streamer, output_scores, return_dict_in_generate,
@@ -541,6 +548,15 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             # torch.manual_seed() makes a run repeatable
             seed = int(torch.randint(0, 2**62, (1,), dtype=torch.int64).item())
             sampling = make_sampling(True, temperature, 1.0 if top_p is None else top_p, 50 if top_k is None else top_k, seed)
+        procs = None
+        if proc_args:
+            # history of row b = the prompt row as passed (placeholders and pad ids included), kept on the device
+            prompt_dev = prompt.to(device=engine.device, dtype=torch.int64).contiguous()
+            procs = [make_logits_proc(prompt_dev[b], proc_args["repetition_penalty"], proc_args["no_repeat_ngram_size"],
+                                      max(proc_args["min_new_tokens"], proc_args["min_length"] - Lt), eos_ids)
+                     for b in range(B)]
+            if all(p is None for p in procs):
+                procs = None
         prof = _StageTimer() if os.environ.get("B2_PROFILE_GENERATE") else None
 
         batcher = self._get_batcher(engine) if B == 1 else None
@@ -559,7 +575,7 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 embeds = engine.splice(prompt.to(torch.int32).reshape(-1).to(engine.device), None, 1, Lt)
                 lens = [Lt]
             self._check_limits(engine, 1, lens[0] + max_new_tokens)
-            req = batcher.submit(embeds, lens[0], sampling, max_new_tokens)
+            req = batcher.submit(embeds, lens[0], sampling, max_new_tokens, proc=procs[0] if procs else None)
             if streamer is not None:
                 streamer.put(prompt.cpu())
             pad = pad_token_id if pad_token_id is not None else (next(iter(eos_ids)) if eos_ids else 0)
@@ -590,13 +606,13 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 self._check_limits(engine, B, max(lens) + max_new_tokens)
                 kv.reset()
                 logits = engine.prefill(kv, embeds, lens, LOGITS_LAST)
-                engine.stream_begin(kv, logits, sampling)
+                engine.stream_begin(kv, logits, sampling, procs)
                 engine.stream_wait(kv, 0, B)          # first sync of this call: every input check has run by now
                 if prof: prof.mark("prefill + first token")
                 return speculative
 
             if plan is not None:
-                self._prefill_reusing(engine, kv, plan, reuse, released_ev, sampling, max_new_tokens)
+                self._prefill_reusing(engine, kv, plan, reuse, released_ev, sampling, max_new_tokens, procs)
                 speculative = False
             else:
                 speculative = prefill(False)
@@ -646,6 +662,32 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             embeds = engine.splice(ids, None, B, Lt)
             lens = [Lt] * B
         return embeds, lens, speculative
+
+    def _logits_processors_on(self):
+        """config.b2_logits_processors or B2_LOGITS_PROCESSORS=1 (off by default, like the other b2_* opt-ins)."""
+        v = getattr(self.config, "b2_logits_processors", None)
+        return bool(v) if v is not None else os.environ.get("B2_LOGITS_PROCESSORS") == "1"
+
+    def _logits_processor_arguments(self, kwargs):
+        """With the opt-in, takes repetition_penalty / no_repeat_ngram_size / min_new_tokens / min_length out of `kwargs` and
+        returns them with their off values filled in, or {} when every one is off. Without it they stay in `kwargs`, where
+        any value other than the off value raises NotImplementedError."""
+        if not self._logits_processors_on():
+            return {}
+        got = {k: kwargs.pop(k) for k in self._LOGITS_PROCESSOR_ARGS if k in kwargs}
+        p = got.get("repetition_penalty")
+        p = 1.0 if p is None else float(p)
+        if not p > 0.0:
+            raise ValueError(f"repetition_penalty has to be a strictly positive float, but is {p}")
+        n = got.get("no_repeat_ngram_size")
+        n = 0 if n is None else int(n)
+        if n < 0:
+            raise ValueError(f"no_repeat_ngram_size has to be a non-negative integer, but is {n}")
+        mnt = int(got.get("min_new_tokens") or 0)
+        ml = int(got.get("min_length") or 0)
+        if p == 1.0 and n == 0 and mnt <= 0 and ml <= 0:
+            return {}
+        return {"repetition_penalty": p, "no_repeat_ngram_size": n, "min_new_tokens": mnt, "min_length": ml}
 
     # ------------------------------------------------------------------ beam search
     def _beam_search_cap(self):
@@ -754,7 +796,7 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             return None
         return {"items": items, "slots": slots, "images": images}
 
-    def _prefill_reusing(self, engine, kv, plan, m, released_ev, sampling, max_new_tokens):
+    def _prefill_reusing(self, engine, kv, plan, m, released_ev, sampling, max_new_tokens, procs=None):
         """Prefill of a planned prompt that keeps the first m spliced rows of `kv`: image slots wholly inside them are not
         encoded, rows [m, L) are spliced on the host-index path and prefilled at position m (b2_prefill_at). m == 0 is an
         ordinary prefill from position 0. Chooses and publishes token 0 like generate()'s own prefill."""
@@ -790,7 +832,7 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         else:
             kv.reset()
             logits = engine.prefill(kv, embeds, None, LOGITS_LAST)
-        engine.stream_begin(kv, logits, sampling)
+        engine.stream_begin(kv, logits, sampling, procs)
         engine.stream_wait(kv, 0, 1)
 
     # ------------------------------------------------------------------ checkpoints
