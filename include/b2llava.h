@@ -235,6 +235,40 @@ int b2_stream_begin_ex(b2_model* m, b2_kv* kv, const float* logits, int B, const
 int b2_stream_enqueue(b2_model* m, b2_kv* kv, int n_steps, void* stream);
 int b2_stream_wait(b2_kv* kv, int index, int32_t* tokens_host, int timeout_ms);
 
+/* Prompt-lookup speculative decoding of one sample (HF generate(prompt_lookup_num_tokens=K, max_matching_ngram_size=n): the draft is
+ * copied from the conversation itself). Every step drafts up to K tokens from the history on the device (the prompt ids, then the
+ * published tokens), runs the pending token and the draft as K + 1 rows of one forward over the weights, and accepts the draft's
+ * leading tokens that equal the tokens selected at the rows before them, plus the token selected after the last match. Row j of
+ * a step is selected (greedy, or the temperature / top-k / top-p draw) as token index t0 + j of the generation, keyed as plain
+ * streaming keys it, so greedy output equals plain decoding's up to the logits' numerics.
+ *   b2_stream_begin_lookup  b2_stream_begin for B == 1 on a bf16 cache. Afterwards b2_stream_enqueue(n) keeps n verify steps in
+ *                           flight: it queues as many as the device has not yet retired below n (read from mapped host memory, no
+ *                           synchronisation), and none once the generation's max_new_tokens are published. Every step publishes at
+ *                           least one token, so token `index` may be waited for (b2_stream_wait) once index < published + steps in
+ *                           flight; a host that calls b2_stream_enqueue(n >= 1) before each b2_stream_wait always may. b2_kv_lengths
+ *                           then reports an upper bound of the cache length. -1 for B != 1, an e4m3 cache, num_tokens outside
+ *                           1..15, max_ngram or max_new_tokens < 1, n_eos outside 0..8, or prompt_len (or the cache length) +
+ *                           max_new_tokens + num_tokens > max_seq. Logits processors cannot be combined with it.
+ *   b2_stream_lookup_stats  the generation's steps that published tokens, the tokens they drafted and the draft tokens accepted
+ *                           (host int32, nullable), as of the last step the device has finished; it does not wait (synchronise the
+ *                           stream first for the final counts).
+ *   b2_decode_rows          the verify forward alone: tokens [R] (host or device, R in 1..16) are appended at slot `slot`'s length
+ *                           (bf16 cache), its length advances by R, logits_out (nullable, host or device) receives fp32 [R, vocab].
+ *                           Rewind with b2_prefill_at's start. */
+typedef struct b2_prompt_lookup {
+    int32_t num_tokens;          /* K: draft tokens per step, 1..15 */
+    int32_t max_ngram;           /* max_matching_ngram_size, >= 1 */
+    int32_t max_new_tokens;      /* the generation publishes at most this many tokens */
+    int32_t n_eos;               /* 0..8: a draft ends before the first eos id */
+    int32_t eos_ids[8];
+    const int64_t* prompt_ids;   /* device, the prompt row as passed (IMAGE_TOKEN_INDEX placeholders end a draft) */
+    int32_t prompt_len;
+} b2_prompt_lookup;
+int b2_stream_begin_lookup(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sampling, const b2_prompt_lookup* lookup,
+                           void* stream);
+int b2_stream_lookup_stats(b2_kv* kv, int32_t* steps, int32_t* drafted, int32_t* accepted);
+int b2_decode_rows(b2_model* m, b2_kv* kv, int slot, const int32_t* tokens, int R, float* logits_out, void* stream);
+
 /* Continuous batching (SURVEY §8f-4: the reference's worker runs up to limit_model_concurrency generate() threads on one
  * model, llava/serve/model_worker.py:230-243, each a batch-1 HF loop; here they share ONE batched decode step). The B slots of
  * a cache are a pool: b2_batch_begin puts the cache in per-slot mode (every slot idle, streaming ring armed);
@@ -342,6 +376,19 @@ int64_t b2_op_decode_attn_scratch_bytes(int B, int H, int nsplit); /* caller zer
  * aligned, Smax % 4 == 0. Appends the quantised row of the new token (bytes and scale) and attends over the stored values. */
 int b2_op_decode_attn_e4m3(const void* qkv, void* k8, void* v8, float* kscale, float* vscale, const int32_t* cur_len, void* out,
                            void* scratch, int B, int H, int Smax, int nsplit, float theta, float scale, void* stream);
+/* multi-query decode attention of the prompt-lookup verify step: qkv [B*R, 3*H*128] with q already roped and rows j < R of sample
+ * b already stored at cache rows cur_len[b] + j (b2_op_rope_kv_write_at with pos0 = cur_len); row j attends cache rows
+ * 0 .. cur_len[b] + j; out [B*R, H*128] bf16. R in 1..16. scratch: b2_op_decode_attn_mq_scratch_bytes, zero-filled once. */
+int b2_op_decode_attn_mq(const void* qkv, const void* kcache, const void* vcache, const int32_t* cur_len, void* out, void* scratch,
+                         int B, int R, int H, int Smax, int nsplit, float scale, void* stream);
+int64_t b2_op_decode_attn_mq_scratch_bytes(int B, int H, int nsplit);
+/* the split factor the verify step uses for b2_op_decode_attn_mq at H heads and a cache of Smax rows (from the kernel's occupancy) */
+int b2_op_decode_attn_mq_nsplit(int H, int Smax);
+/* the draft of one prompt-lookup step: hist device int32 [len] (the last id is the pending token), max_length = prompt length +
+ * max_new_tokens of the generation; out_tokens device int32 [num_tokens + 1] = pending, draft, padding; out_draft_len device int32.
+ * Synchronises the stream. */
+int b2_op_prompt_lookup(const int32_t* hist, int len, int num_tokens, int max_ngram, int max_length, const int32_t* eos_host, int n_eos,
+                        int V, int32_t* out_tokens, int32_t* out_draft_len, void* stream);
 /* the split-KV factor a decode step uses for this shape and cache format (from the resident CTAs per SM of the kernel it launches) */
 int b2_op_decode_attn_nsplit(int B, int H, int Smax, int kv_dtype);
 /* prefill's cache write of an e4m3 cache: kstage / vstage [B,H,S,128] bf16 (roped K, V of one layer) -> rows t < seq_lens[b]

@@ -515,6 +515,233 @@ __global__ void __launch_bounds__(DA_THREADS) decode_attn_kernel(DecodeAttnParam
 }
 
 // ------------------------------------------------------------------------------------------------
+// multi-query decode attention (the prompt-lookup verify step): R <= 16 query rows of one sample, row j at position
+// len + j attending cache rows 0 .. len + j. The rows' own K / V are already in the cache and q is roped in place in qkv
+// (rope_kv_write at pos0 = cur_len). grid (nsplit, H, B), 128 threads. Each 64-key tile of the split's range is loaded
+// once (cp.async, double-buffered) and serves every query row: the 16 rows are one mma.sync m16n8k16 A tile for QK^T and
+// for PV, warp w takes keys [16w, 16w + 16) of each tile with its own fp32 online softmax. The four warps merge in shared
+// memory, and the last CTA of a (b, head) merges the splits in split order, as decode_attn_kernel does.
+// ------------------------------------------------------------------------------------------------
+constexpr int MQ_ROWS = 16;
+constexpr int MQ_BN = 64;
+constexpr int MQ_LD = DA_D + 8;  // padded smem row: conflict-free ldmatrix
+constexpr size_t MQ_SMEM = (size_t)(MQ_ROWS + 4 * MQ_BN) * MQ_LD * sizeof(__nv_bfloat16);
+
+struct DecodeAttnMqParams {
+    const __nv_bfloat16* qkv;  // [B*R, 3*H*128], q roped
+    const __nv_bfloat16* kcache;
+    const __nv_bfloat16* vcache;
+    const int32_t* cur_len;    // [B]: position of row 0
+    __nv_bfloat16* out;        // [B*R, H*128]
+    float* partial;            // [B*H*nsplit][16][128 + 2]
+    int32_t* counters;         // [B*H]
+    int R, H, Smax, nsplit;
+    float scale_log2;
+};
+
+__global__ void __launch_bounds__(128) decode_attn_mq_kernel(DecodeAttnMqParams p) {
+    extern __shared__ __align__(16) uint8_t mq_smem[];
+    __nv_bfloat16* sQ = reinterpret_cast<__nv_bfloat16*>(mq_smem);  // [16][LD]
+    __nv_bfloat16* sK = sQ + MQ_ROWS * MQ_LD;                         // [2][64][LD]
+    __nv_bfloat16* sV = sK + 2 * MQ_BN * MQ_LD;                       // [2][64][LD]
+    __shared__ int s_last;
+    const int split = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    pdl_trigger();
+    pdl_wait();  // qkv (rope_kv_write) and cur_len are upstream outputs
+    const int R = p.R, len = p.cur_len[b];
+    const int total = len + R;  // keys the last row attends
+    const int hd = p.H * DA_D;
+    const int chunk = (total + p.nsplit - 1) / p.nsplit;
+    const int k_begin = min(split * chunk, total), k_end = min(k_begin + chunk, total);
+    const int n_tiles = (k_end - k_begin + MQ_BN - 1) / MQ_BN;
+
+    const size_t cbase = ((size_t)b * p.H + head) * p.Smax * DA_D;
+    const __nv_bfloat16* kg = p.kcache + cbase;
+    const __nv_bfloat16* vg = p.vcache + cbase;
+    const __nv_bfloat16* qg = p.qkv + (size_t)b * R * 3 * hd + head * DA_D;
+    constexpr int CH = DA_D / 8;  // 16-byte chunks per row
+    for (int i = tid; i < MQ_ROWS * CH; i += 128) {
+        const int r = i / CH, c = i % CH;
+        cp_async_16(sQ + r * MQ_LD + c * 8, qg + (size_t)min(r, R - 1) * 3 * hd + c * 8, r < R);  // rows >= R are zero
+    }
+    auto load_kv = [&](int tile, int buf) {
+        for (int i = tid; i < MQ_BN * CH; i += 128) {
+            const int r = i / CH, c = i % CH;
+            const int t = k_begin + tile * MQ_BN + r;
+            const bool ok = t < k_end;
+            const size_t off = (size_t)(ok ? t : 0) * DA_D + c * 8;
+            cp_async_16(sK + (buf * MQ_BN + r) * MQ_LD + c * 8, kg + off, ok);
+            cp_async_16(sV + (buf * MQ_BN + r) * MQ_LD + c * 8, vg + off, ok);
+        }
+    };
+    if (n_tiles > 0) load_kv(0, 0);
+    cp_async_commit();
+
+    uint32_t qf[DA_D / 16][4];
+    float oacc[DA_D / 8][4];
+#pragma unroll
+    for (int i = 0; i < DA_D / 8; ++i) oacc[i][0] = oacc[i][1] = oacc[i][2] = oacc[i][3] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY};
+    float l_run[2] = {0.f, 0.f};
+    const int g = lane >> 2, tq = lane & 3;  // this thread's query rows: g and g + 8
+
+    for (int j = 0; j < n_tiles; ++j) {
+        if (j + 1 < n_tiles) load_kv(j + 1, (j + 1) & 1);
+        cp_async_commit();
+        cp_async_wait<1>();
+        __syncthreads();
+        if (j == 0) {
+#pragma unroll
+            for (int kk = 0; kk < DA_D / 16; ++kk)
+                ldmatrix_x4(qf[kk], sQ + ((lane & 7) + ((lane >> 3) & 1) * 8) * MQ_LD + kk * 16 + (lane >> 4) * 8);
+        }
+        const __nv_bfloat16* tK = sK + ((j & 1) * MQ_BN + warp * 16) * MQ_LD;
+        const __nv_bfloat16* tV = sV + ((j & 1) * MQ_BN + warp * 16) * MQ_LD;
+
+        // ---- S = Q K^T over this warp's 16 keys ----
+        float s[2][4];
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt) s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
+#pragma unroll
+        for (int kk = 0; kk < DA_D / 16; ++kk) {
+            uint32_t bfr[4];
+            ldmatrix_x4(bfr, tK + ((lane & 7) + (lane >> 4) * 8) * MQ_LD + kk * 16 + ((lane >> 3) & 1) * 8);
+            mma_bf16_16816(s[0], qf[kk], bfr[0], bfr[1]);
+            mma_bf16_16816(s[1], qf[kk], bfr[2], bfr[3]);
+        }
+
+        // ---- scale, per-row causal limit, online softmax (fp32, log2 domain) ----
+        const int key0 = k_begin + j * MQ_BN + warp * 16;
+        float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int key = key0 + nt * 8 + tq * 2 + (e & 1);
+                const int row = g + (e >> 1) * 8;
+                const bool ok = key < k_end && key <= len + row;
+                const float val = ok ? s[nt][e] * p.scale_log2 : -INFINITY;
+                s[nt][e] = val;
+                mx[e >> 1] = fmaxf(mx[e >> 1], val);
+            }
+        }
+        float corr[2], m_use[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+            mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+            const float m_new = fmaxf(m_run[h], mx[h]);
+            m_use[h] = (m_new == -INFINITY) ? 0.f : m_new;
+            corr[h] = exp2f(m_run[h] - m_use[h]);
+            m_run[h] = m_new;
+            l_run[h] *= corr[h];
+        }
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float pv = exp2f(s[nt][e] - m_use[e >> 1]);
+                s[nt][e] = pv;
+                l_run[e >> 1] += pv;
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < DA_D / 8; ++i) {
+            oacc[i][0] *= corr[0]; oacc[i][1] *= corr[0];
+            oacc[i][2] *= corr[1]; oacc[i][3] *= corr[1];
+        }
+
+        // ---- O += P V, with P = hi + lo as two bf16 operands: p keeps ~16 significant bits, close to decode_attn's fp32 p ----
+        uint32_t pa[4], pl[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const float x0 = s[i >> 1][(i & 1) * 2], x1 = s[i >> 1][(i & 1) * 2 + 1];
+            pa[i] = pack_bf16(x0, x1);
+            pl[i] = pack_bf16(x0 - bf16_lo(pa[i]), x1 - bf16_hi(pa[i]));
+        }
+#pragma unroll
+        for (int dp = 0; dp < DA_D / 16; ++dp) {
+            uint32_t bfr[4];
+            ldmatrix_x4_trans(bfr, tV + ((lane & 7) + ((lane >> 3) & 1) * 8) * MQ_LD + dp * 16 + (lane >> 4) * 8);
+            mma_bf16_16816(oacc[2 * dp], pa, bfr[0], bfr[1]);
+            mma_bf16_16816(oacc[2 * dp + 1], pa, bfr[2], bfr[3]);
+            mma_bf16_16816(oacc[2 * dp], pl, bfr[0], bfr[1]);
+            mma_bf16_16816(oacc[2 * dp + 1], pl, bfr[2], bfr[3]);
+        }
+        __syncthreads();  // buffer (j & 1) is refilled at iteration j + 1
+    }
+    cp_async_wait<0>();
+    __syncthreads();
+
+    // ---- merge the four warps (the K tiles' shared memory is free now) ----
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
+        l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
+    }
+    float* s_o = reinterpret_cast<float*>(sK);   // [4][16][128]
+    float* s_ml = reinterpret_cast<float*>(sV);  // [4][16][2]
+#pragma unroll
+    for (int i = 0; i < DA_D / 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+            s_o[(warp * MQ_ROWS + g + (e >> 1) * 8) * DA_D + i * 8 + tq * 2 + (e & 1)] = oacc[i][e];
+    if (tq == 0)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            s_ml[(warp * MQ_ROWS + g + h * 8) * 2] = m_run[h];
+            s_ml[(warp * MQ_ROWS + g + h * 8) * 2 + 1] = l_run[h];
+        }
+    __syncthreads();
+    const int bh = b * p.H + head;
+    for (int r = 0; r < R; ++r) {  // thread tid owns output column tid
+        float m_cta = -INFINITY;
+#pragma unroll
+        for (int w = 0; w < 4; ++w) m_cta = fmaxf(m_cta, s_ml[(w * MQ_ROWS + r) * 2]);
+        float l_cta = 0.f, o_cta = 0.f;
+#pragma unroll
+        for (int w = 0; w < 4; ++w) {
+            const float mw = s_ml[(w * MQ_ROWS + r) * 2];
+            const float wt = (mw == -INFINITY) ? 0.f : exp2f(mw - m_cta);
+            l_cta += s_ml[(w * MQ_ROWS + r) * 2 + 1] * wt;
+            o_cta += s_o[(w * MQ_ROWS + r) * DA_D + tid] * wt;
+        }
+        float* part = p.partial + (((size_t)bh * p.nsplit + split) * MQ_ROWS + r) * (DA_D + 2);
+        part[tid] = o_cta;
+        if (tid == 0) { part[DA_D] = m_cta; part[DA_D + 1] = l_cta; }
+    }
+
+    // ---- last CTA of this (b, head) merges the splits ----
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) {
+        const int prev = atomicAdd(&p.counters[bh], 1);
+        s_last = (prev == p.nsplit - 1) ? 1 : 0;
+    }
+    __syncthreads();
+    if (s_last) {
+        __threadfence();
+        for (int r = 0; r < R; ++r) {
+            const float* pb = p.partial + ((size_t)bh * p.nsplit * MQ_ROWS + r) * (DA_D + 2);
+            const size_t stride = (size_t)MQ_ROWS * (DA_D + 2);
+            float m_all = -INFINITY;
+            for (int s = 0; s < p.nsplit; ++s) m_all = fmaxf(m_all, __ldcg(pb + s * stride + DA_D));
+            float l_all = 0.f, o_all = 0.f;
+#pragma unroll 4
+            for (int s = 0; s < p.nsplit; ++s) {
+                const float ms = __ldcg(pb + s * stride + DA_D);
+                const float wt = (ms == -INFINITY) ? 0.f : exp2f(ms - m_all);
+                l_all += __ldcg(pb + s * stride + DA_D + 1) * wt;
+                o_all += __ldcg(pb + s * stride + tid) * wt;
+            }
+            p.out[((size_t)b * R + r) * hd + head * DA_D + tid] = __float2bfloat16_rn(o_all / l_all);
+        }
+        if (tid == 0) p.counters[bh] = 0;  // self-reset for the next launch
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // e4m3 KV cache. A cache row is one head of one token: 128 e4m3 bytes + one fp32 scale (amax / 448, 1 for a zero row;
 // the rule of quant_fp8.cu over the 128 elements of the row). K is quantised after RoPE.
 // ------------------------------------------------------------------------------------------------
@@ -919,6 +1146,47 @@ int decode_attn_bf16(const DecodeAttnArgs& a, cudaStream_t stream) {
     p.scale_log2 = a.scale * 1.4426950408889634f;
     dim3 grid(a.nsplit, a.H, a.B);
     B2_CUDA_CHECK(launch_pdl(decode_attn_kernel, grid, dim3(DA_THREADS), 0, stream, p));
+    B2_LAUNCH_CHECK();
+    return 0;
+}
+
+// resident CTAs of decode_attn_mq_kernel per SM (shared-memory-limited: 74 KB of K / V tiles per CTA), for the split heuristic
+int decode_attn_mq_ctas_per_sm() {
+    static int occ = 0;
+    if (occ == 0) {
+        int n = 0;
+        if (cudaFuncSetAttribute(decode_attn_mq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MQ_SMEM) != cudaSuccess ||
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, decode_attn_mq_kernel, 128, MQ_SMEM) != cudaSuccess || n < 1) {
+            cudaGetLastError();
+            n = 3;
+        }
+        occ = n;
+    }
+    return occ;
+}
+
+size_t decode_attn_mq_scratch_bytes(int B, int H, int nsplit) {
+    return (size_t)B * H * nsplit * MQ_ROWS * (DA_D + 2) * sizeof(float) + (size_t)B * H * sizeof(int32_t);
+}
+
+int decode_attn_mq_bf16(const DecodeAttnArgs& a, cudaStream_t stream) {
+    B2_CHECK_ARG(a.D == DA_D, "decode_attn_mq: head_dim must be 128 (got %d)", a.D);
+    B2_CHECK_ARG(a.R >= 1 && a.R <= MQ_ROWS, "decode_attn_mq: %d query rows (1..%d)", a.R, MQ_ROWS);
+    B2_CHECK_ARG(a.nsplit >= 1 && a.B > 0 && a.H > 0, "decode_attn_mq: bad launch shape");
+    B2_CHECK_ARG(((reinterpret_cast<uintptr_t>(a.qkv) | reinterpret_cast<uintptr_t>(a.kcache) |
+                   reinterpret_cast<uintptr_t>(a.vcache)) & 15) == 0, "decode_attn_mq: buffers must be 16-byte aligned");
+    decode_attn_mq_ctas_per_sm();  // sets the dynamic shared-memory attribute
+    DecodeAttnMqParams p;
+    p.qkv = reinterpret_cast<const __nv_bfloat16*>(a.qkv);
+    p.kcache = reinterpret_cast<const __nv_bfloat16*>(a.kcache);
+    p.vcache = reinterpret_cast<const __nv_bfloat16*>(a.vcache);
+    p.cur_len = a.cur_len;
+    p.out = reinterpret_cast<__nv_bfloat16*>(a.out);
+    p.partial = a.partial;
+    p.counters = a.counters;
+    p.R = a.R; p.H = a.H; p.Smax = a.Smax; p.nsplit = a.nsplit;
+    p.scale_log2 = a.scale * 1.4426950408889634f;
+    B2_CUDA_CHECK(launch_pdl(decode_attn_mq_kernel, dim3(a.nsplit, a.H, a.B), dim3(128), MQ_SMEM, stream, p));
     B2_LAUNCH_CHECK();
     return 0;
 }

@@ -161,9 +161,17 @@ struct DecodeAttnArgs {
     int32_t* counters = nullptr;                     // workspace [B*H], zero-initialised, self-resetting
     int B = 0, H = 0, D = 128, Smax = 0, nsplit = 1;
     float theta = 10000.f, scale = 1.f;
+    int R = 1;  // decode_attn_mq only: query rows per sample
 };
 int decode_attn_ctas_per_sm();
 int decode_attn_bf16(const DecodeAttnArgs& a, cudaStream_t stream);
+// multi-query decode (prompt-lookup verify step) over a bf16 cache: qkv [B*R, 3*H*D] with q already roped and the R rows'
+// K / V already stored at cache rows cur_len[b] .. cur_len[b] + R - 1 (rope_kv_write at pos0 = cur_len); row j attends rows
+// 0 .. cur_len[b] + j; out [B*R, H*D]. R <= 16. partial: [B*H*nsplit*16*(D+2)] fp32; counters as decode_attn's. The cache
+// length is not advanced. No RoPE, no cache write.
+int decode_attn_mq_ctas_per_sm();
+size_t decode_attn_mq_scratch_bytes(int B, int H, int nsplit);  // partial then counters
+int decode_attn_mq_bf16(const DecodeAttnArgs& a, cudaStream_t stream);
 // the same step over an e4m3 cache (rows of 128 bytes + one fp32 scale per row); Smax % 4 == 0
 int decode_attn_e4m3_ctas_per_sm();
 int decode_attn_e4m3(const DecodeAttnArgs& a, cudaStream_t stream);
@@ -254,15 +262,42 @@ struct ProcState {
     uint32_t* bits;
     int cap, words;
 };
+// Prompt-lookup speculative decoding of one sample (b2_stream_begin_lookup), device-resident so the verify step is a CUDA
+// graph: prompt_lookup drafts from the history, the verify forward runs R = K + 1 rows, sample_publish's multi-row mode accepts.
+constexpr int kSpecMaxRows = 16;
+struct SpecState {
+    int K;                    // draft tokens per step (R = K + 1 rows)
+    int ngram;                // max_matching_ngram_size
+    int max_new;              // the generation never publishes more tokens
+    int n_eos;
+    int eos[kProcMaxEos];     // a draft ends before the first eos id
+    int prompt_len;
+    int hist_len;             // history (ProcState row 0) = the prompt, then every published token but the pending one (tok[0])
+    int draft_len;            // draft of the step in flight (rows[1 .. draft_len])
+    int32_t rows[kSpecMaxRows];  // the step's input tokens: the pending token, the draft, padding
+    int steps, drafted, accepted;  // steps that published tokens, tokens they drafted, draft tokens accepted
+    int retired;              // verify steps finished, including those queued after the generation was complete
+    int32_t sel[kSpecMaxRows];  // token selected from each row's logits
+    int* mirror;              // mapped host int[6]: steps, drafted, accepted, cache length, retired, tokens published
+};
+// one CTA: history hist[0, hist_len) + tok[0] -> draft (HF PromptLookupCandidateGenerator.get_candidates, cut before the first eos
+// id or id outside [0, V)) -> spec->rows = tok[0], the draft, tok[0] as padding up to R; spec->draft_len. st->pub_counter = tokens
+// published so far.
+int prompt_lookup(int32_t* hist, SpecState* spec, const SampleState* st, const int32_t* tok, int V, int R, cudaStream_t stream);
+
 enum { SP_SELECT = 1,     // choose from `logits` (argmax or sample) and write tok[b]; otherwise tok[b] is already chosen
        SP_WRITE_OUT = 2,  // out_tokens[(*step_counter + step_offset) * B + b] = token
        SP_BUMP = 4 };     // last row: *step_counter += 1, cur_len[b] += 1
 int sample_state_set(SampleState* st_dev, const SampleState& v, cudaStream_t stream);
 // `proc` processes rows whose ProcRow is on (and appends the chosen token to their history); `processed_out` (nullable, fp32
-// [B,V]) receives each selected row's logits after processing and before temperature
+// [B,V]) receives each selected row's logits after processing and before temperature.
+// With `spec` (multi-row acceptance of a verify step, sample 0 only): the B rows are the step's R rows; row j is selected as
+// draw pub_counter + j (Philox row 0, as plain streaming keys it) unless j > draft_len; the last CTA accepts n = matches + 1
+// tokens (HF's n_matches rule, capped by max_new), appends them to the history (proc.hist row 0), publishes them at ring indices
+// pub_counter .. + n - 1, sets tok[0] to the last one and advances cur_len[0] and pub_counter by n. flags must be SP_SELECT.
 int sample_publish(const float* logits, int V, int B, SampleState* st_dev, RowState* rows_dev, int32_t* tok, int32_t* out_tokens,
                    int32_t* step_counter, int32_t* cur_len, int32_t* ring_dev, int ring_cap, int flags, int step_offset,
-                   const ProcState& proc, float* processed_out, cudaStream_t stream);
+                   const ProcState& proc, float* processed_out, cudaStream_t stream, SpecState* spec = nullptr);
 // row := v, its history := ids[0, len) (int64, device) followed by `first_token` when >= 0, and its bitmap rebuilt from those ids
 int proc_seed(const ProcState& proc, int row, const ProcRow& v, const int64_t* ids, int len, int first_token, int V,
               cudaStream_t stream);

@@ -187,6 +187,19 @@ struct b2_kv {
     DevBuf proc_rows, proc_hist, proc_bits;
     std::vector<char> proc_on;  // host copy of ProcRow::on per slot
     bool any_proc() const { for (char c : proc_on) if (c) return true; return false; }
+    // prompt-lookup speculative decoding (b2_stream_begin_lookup / b2_decode_rows; allocated by the first call): SpecState, the
+    // verify forward's logits fp32 [16][V], decode_attn_mq's partials and counters, a mapped host mirror of the step counters,
+    // and one captured verify step per row count R. The history lives in proc_hist row 0.
+    DevBuf spec_state, spec_logits, spec_attn;
+    int* spec_mirror = nullptr;  // cudaHostAlloc(mapped) int[6]: SpecState::mirror
+    int spec_nsplit = 0;
+    int spec_R = 0;              // rows of the lookup generation in progress (0: none)
+    int spec_max_new = 0;
+    int spec_queued = 0;         // verify steps queued in the generation
+    int spec_len0 = 0;           // cache length when it began
+    std::array<cudaGraphExec_t, kSpecMaxRows + 1> spec_graph{};
+    std::array<int, kSpecMaxRows + 1> spec_launches{};
+    std::array<char, kSpecMaxRows + 1> spec_warm{};
     bool counted = false;  // included in m->kv_live
     bool e4m3() const { return dtype == B2_KV_E4M3; }
     size_t elem_bytes() const { return e4m3() ? 1 : 2; }
@@ -790,6 +803,72 @@ int decode_step_run(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     return 0;
 }
 
+// ---- prompt-lookup speculative decoding ----------------------------------------------------------------------------------
+int32_t* spec_rows(b2_kv* kv) { return reinterpret_cast<int32_t*>(kv->spec_state.as<char>() + offsetof(SpecState, rows)); }
+
+// The verify forward of R rows of slot `slot` (bf16 cache): tokens spec->rows -> K / V at cache rows len .. len + R - 1 of every
+// layer -> logits fp32 [R, V] in kv->spec_logits. Every Linear runs at R rows on decode_plan(m, kv, R)'s path; the cache length is
+// not advanced.
+int rows_forward(b2_model* m, b2_kv* kv, int slot, int R, cudaStream_t st) {
+    const b2_model_desc& d = m->d;
+    const int h = d.hidden, I = d.inter, H = d.heads, V = d.vocab;
+    const DecodePlan plan = decode_plan(m, kv, R);
+    const DecodePath p = plan.layer;
+    const int32_t* len = kv->len_dev.as<int32_t>() + slot;
+    const size_t slot_off = (size_t)slot * H * kv->pitch * m->hd * kv->elem_bytes();
+    const size_t attn_partial = decode_attn_mq_scratch_bytes(1, H, kv->spec_nsplit) - (size_t)H * sizeof(int32_t);
+    B2_TRY(embed_tokens(spec_rows(kv), m->embed.p, m->x.p, R, h, V, m->err_dev, st));
+    for (int l = 0; l < d.layers; ++l) {
+        LlamaLayer& L = m->ll[l];
+        LayerW lw = {};
+        if (p != GEMV_NF4) B2_TRY(layer_weights(m, l, &lw, st));
+        B2_TRY(decode_linear(m, kv, p, L.qkv, lw.wqkv, m->x.p, h, L.ln1.p, false, m->qkv.p, 3 * h, 0, R, 3 * h, h, ACT_NONE, st));
+        B2_TRY(rope_kv_write(m->qkv.p, kv->k_layer(l) + slot_off, kv->v_layer(l) + slot_off, 1, R, H, m->hd, kv->pitch,
+                             d.rope_theta, st, len));
+        DecodeAttnArgs da;
+        da.qkv = m->qkv.p;
+        da.kcache = kv->k_layer(l) + slot_off;
+        da.vcache = kv->v_layer(l) + slot_off;
+        da.cur_len = len;
+        da.out = m->attn.p;
+        da.partial = kv->spec_attn.as<float>();
+        da.counters = reinterpret_cast<int32_t*>(kv->spec_attn.as<char>() + attn_partial);
+        da.B = 1; da.R = R; da.H = H; da.D = m->hd; da.Smax = kv->pitch; da.nsplit = kv->spec_nsplit;
+        da.scale = 1.0f / sqrtf((float)m->hd);
+        B2_TRY(decode_attn_mq_bf16(da, st));
+        B2_TRY(decode_linear(m, kv, p, L.o, lw.wo, m->attn.p, h, nullptr, true, m->x.p, h, 0, R, h, h, ACT_NONE, st));
+        B2_TRY(decode_linear(m, kv, p, L.gu, lw.wgu, m->x.p, h, L.ln2.p, false, m->act.p, I, 0, R, 2 * I, h, ACT_SWIGLU, st));
+        B2_TRY(decode_linear(m, kv, p, L.d, lw.wd, m->act.p, I, nullptr, true, m->x.p, h, 0, R, h, I, ACT_NONE, st));
+    }
+    return decode_linear(m, kv, plan.head, m->head, m->head.w.p, m->x.p, h, m->final_norm.p, false, kv->spec_logits.p, V, 1, R, V,
+                         h, ACT_NONE, st);
+}
+
+// one verify step of the lookup generation on slot 0: draft -> forward of the R rows -> acceptance (publication, history, length)
+int verify_step_launch(b2_model* m, b2_kv* kv, int R, cudaStream_t st) {
+    SpecState* spec = kv->spec_state.as<SpecState>();
+    SampleState* sst = kv->sstate.as<SampleState>();
+    B2_TRY(prompt_lookup(kv->proc_hist.as<int32_t>(), spec, sst, kv->tok.as<int32_t>(), m->d.vocab, R, st));
+    B2_TRY(rows_forward(m, kv, 0, R, st));
+    return sample_publish(kv->spec_logits.as<float>(), m->d.vocab, R, sst, nullptr, kv->tok.as<int32_t>(), nullptr,
+                          kv->step_counter.as<int32_t>(), kv->len_dev.as<int32_t>(), kv->ring_dev, kv->ring_cap, SP_SELECT, 0,
+                          proc_state(kv), nullptr, st, spec);
+}
+
+// the verify step through its CUDA graph (one per R): the first step at an R runs eagerly, the second captures, later ones replay
+int verify_step_run(b2_model* m, b2_kv* kv, int R, cudaStream_t st) {
+    if (!kv->spec_warm[R]) {
+        B2_TRY(verify_step_launch(m, kv, R, st));
+        kv->spec_warm[R] = 1;
+        return 0;
+    }
+    if (kv->spec_graph[R] == nullptr)
+        B2_TRY(capture_graph(st, &kv->spec_graph[R], &kv->spec_launches[R], [&] { return verify_step_launch(m, kv, R, st); }));
+    B2_CUDA_CHECK(cudaGraphLaunch(kv->spec_graph[R], st));
+    g_launch_count += (unsigned long long)kv->spec_launches[R];
+    return 0;
+}
+
 // makes `dev` current for the duration of an ABI call and restores the caller's device afterwards
 struct DeviceGuard {
     int prev = -1;
@@ -834,7 +913,7 @@ int b2_init(int device) {
 }
 
 const char* b2_last_error(void) { return g_err; }
-int b2_version(void) { return 6; }
+int b2_version(void) { return 7; }
 unsigned long long b2_launch_count(void) { return g_launch_count; }
 
 int b2_model_create(const b2_model_desc* desc, b2_model** out) {
@@ -1287,12 +1366,15 @@ int b2_kv_destroy(b2_kv* kv) {
     if (kv->counted) kv->m->kv_live--;
     if (kv->ring_host) cudaFreeHost(kv->ring_host);
     if (kv->graph) cudaGraphExecDestroy(kv->graph);
+    for (cudaGraphExec_t g : kv->spec_graph) if (g) cudaGraphExecDestroy(g);
+    if (kv->spec_mirror) cudaFreeHost(kv->spec_mirror);
     if (kv->own_stream) cudaStreamDestroy(kv->own_stream);
     if (kv->ev_fork) cudaEventDestroy(kv->ev_fork);
     if (kv->ev_join) cudaEventDestroy(kv->ev_join);
     DevBuf* bs[] = {&kv->k, &kv->v, &kv->kscale, &kv->vscale, &kv->len_dev, &kv->tok, &kv->step_counter, &kv->out_tokens, &kv->attn_partial,
                     &kv->attn_counters, &kv->mega_layers, &kv->mega_sync, &kv->sk_partial, &kv->sk_counters, &kv->sstate, &kv->rows_dev, &kv->rope_tab,
-                    &kv->beam_in, &kv->beam_ws, &kv->beam_out, &kv->proc_rows, &kv->proc_hist, &kv->proc_bits};
+                    &kv->beam_in, &kv->beam_ws, &kv->beam_out, &kv->proc_rows, &kv->proc_hist, &kv->proc_bits,
+                    &kv->spec_state, &kv->spec_logits, &kv->spec_attn};
     for (DevBuf* b : bs) b->free();
     delete kv;
     return 0;
@@ -1554,6 +1636,7 @@ static int set_greedy_unpublished(b2_kv* kv, cudaStream_t st) {
     SampleState v = {};
     v.temperature = 1.f; v.top_p = 1.f;
     kv->stream_B = 0;  // any streaming generation on this cache is over
+    kv->spec_R = 0;
     B2_TRY(proc_all_off(kv, st));
     return set_sampling(kv, v, false, st);
 }
@@ -1615,6 +1698,55 @@ static int proc_set_row(b2_kv* kv, int row, const ProcRow& v, const int64_t* ids
     kv->proc_on[row] = 1;
     return 0;
 }
+// The lookup state of a bf16 cache, allocated on first use (b2_kv_bytes does not count it), and a stream-K workspace for R rows
+// when decode_plan takes SKINNY there. A workspace that grows is reallocated, so graphs captured over the old one are dropped.
+static int spec_alloc(b2_model* m, b2_kv* kv, int R, cudaStream_t st) {
+    B2_CHECK_ARG(!kv->e4m3(), "prompt lookup: the verify step reads a bf16 KV cache (this one is e4m3)");
+    B2_CHECK_ARG(R >= 1 && R <= kSpecMaxRows, "prompt lookup: %d rows per step (1..%d)", R, kSpecMaxRows);
+    B2_CHECK_ARG(!m->fp8_decode || R <= m->d.max_batch, "prompt lookup: %d rows exceed the e4m3 activation buffer (model max_batch %d)",
+                 R, m->d.max_batch);
+    B2_TRY(proc_alloc(kv, st));
+    if (kv->spec_state.p == nullptr) {
+        const int H = m->d.heads;
+        const int nsplit = decode_nsplit(1, H, kv->max_seq, decode_attn_mq_ctas_per_sm());
+        const size_t attn = decode_attn_mq_scratch_bytes(1, H, nsplit);
+        int r = kv->spec_state.alloc(sizeof(SpecState));
+        if (r == 0) r = kv->spec_logits.alloc((size_t)kSpecMaxRows * m->d.vocab * sizeof(float));
+        if (r == 0) r = kv->spec_attn.alloc(attn);
+        if (r == 0 && (cudaHostAlloc(reinterpret_cast<void**>(&kv->spec_mirror), 6 * sizeof(int), cudaHostAllocMapped) != cudaSuccess ||
+                       cudaMemsetAsync(kv->spec_attn.p, 0, attn, st) != cudaSuccess)) {
+            set_error("prompt lookup: %s", cudaGetErrorString(cudaGetLastError()));
+            r = -2;
+        }
+        if (r != 0) {
+            kv->spec_state.free(); kv->spec_logits.free(); kv->spec_attn.free();
+            if (kv->spec_mirror) { cudaFreeHost(kv->spec_mirror); kv->spec_mirror = nullptr; }
+            return r;
+        }
+        memset(kv->spec_mirror, 0, 6 * sizeof(int));
+        kv->spec_nsplit = nsplit;
+    }
+    if (R >= 7) {  // use_skinny's batches: the stream-K GEMM needs its workspace at R rows
+        size_t ws = 0;
+        int nmax = 0;
+        for (const LinearShape& sh : layer_shapes(m->d)) { ws = std::max(ws, gemm_skinny_workspace_bytes(R, sh.N, sh.K)); nmax = std::max(nmax, sh.N); }
+        ws = std::max(ws, gemm_skinny_workspace_bytes(R, m->d.vocab, m->d.hidden));
+        nmax = std::max(nmax, m->d.vocab);
+        if (kv->sk_partial.bytes < ws || kv->sk_counters.bytes < gemm_skinny_counter_bytes(nmax)) {
+            B2_CUDA_CHECK(cudaStreamSynchronize(st));
+            if (kv->graph) { cudaGraphExecDestroy(kv->graph); kv->graph = nullptr; kv->graph_B = 0; }
+            for (cudaGraphExec_t& g : kv->spec_graph) if (g) { cudaGraphExecDestroy(g); g = nullptr; }
+            const size_t cb = gemm_skinny_counter_bytes(nmax);
+            kv->sk_partial.free(); kv->sk_counters.free();
+            int r = kv->sk_partial.alloc(ws);
+            if (r == 0) r = kv->sk_counters.alloc(cb);
+            if (r != 0) { kv->sk_partial.free(); kv->sk_counters.free(); return r; }
+            B2_CUDA_CHECK(cudaMemsetAsync(kv->sk_counters.p, 0, cb, st));
+        }
+    }
+    return 0;
+}
+
 static bool is_device_pointer(const void* p) {
     cudaPointerAttributes attr;
     if (cudaPointerGetAttributes(&attr, p) != cudaSuccess) { cudaGetLastError(); return false; }
@@ -1817,6 +1949,7 @@ int b2_stream_begin_ex(b2_model* m, b2_kv* kv, const float* logits, int B, const
     for (int b = 0; b < B; ++b) B2_TRY(proc_row_of(proc ? proc + b : nullptr, kv->max_seq + 1, &pr[b], "b2_stream_begin_ex"));
     kv->epoch += 1;
     v.tag = 1 + kv->epoch % 2047;
+    kv->spec_R = 0;
     B2_TRY(ws_enter(m, st));
     B2_TRY(set_sampling(kv, v, true, st));
     B2_CUDA_CHECK(cudaMemsetAsync(kv->step_counter.p, 0, 4, st));
@@ -1831,11 +1964,135 @@ int b2_stream_begin_ex(b2_model* m, b2_kv* kv, const float* logits, int B, const
     return ws_leave(m, st);
 }
 
+int b2_stream_begin_lookup(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sp, const b2_prompt_lookup* lk,
+                           void* stream) {
+    B2_CHECK_ARG(m && kv && logits && lk && kv->m == m, "b2_stream_begin_lookup: bad handle");
+    B2_CHECK_ARG(m->finalized, "b2_stream_begin_lookup: model not finalized");
+    B2_CHECK_ARG(B == 1, "b2_stream_begin_lookup: prompt lookup decodes one sample (B=%d)", B);
+    B2_CHECK_ARG(!kv->e4m3(), "b2_stream_begin_lookup: the verify step reads a bf16 KV cache");
+    B2_CHECK_ARG(lk->num_tokens >= 1 && lk->num_tokens < kSpecMaxRows, "b2_stream_begin_lookup: num_tokens %d outside 1..%d",
+                 lk->num_tokens, kSpecMaxRows - 1);
+    B2_CHECK_ARG(lk->max_ngram >= 1 && lk->max_new_tokens >= 1, "b2_stream_begin_lookup: max_ngram and max_new_tokens must be >= 1");
+    B2_CHECK_ARG(lk->n_eos >= 0 && lk->n_eos <= kProcMaxEos, "b2_stream_begin_lookup: n_eos must be in [0, %d]", kProcMaxEos);
+    B2_CHECK_ARG(lk->prompt_len >= 0 && (lk->prompt_len == 0 || lk->prompt_ids != nullptr), "b2_stream_begin_lookup: bad prompt ids");
+    B2_CHECK_ARG((int64_t)lk->prompt_len + lk->max_new_tokens + lk->num_tokens <= kv->max_seq,
+                 "b2_stream_begin_lookup: prompt %d + max_new_tokens %d + num_tokens %d exceed the cache's max_seq %d", lk->prompt_len,
+                 lk->max_new_tokens, lk->num_tokens, kv->max_seq);
+    SampleState v = {};
+    v.temperature = 1.f; v.top_p = 1.f;
+    if (sp != nullptr && sp->do_sample) {
+        B2_CHECK_ARG(sp->temperature > 0.f && sp->top_p > 0.f && sp->top_p <= 1.f && sp->top_k >= 0, "b2_stream_begin_lookup: bad sampling parameters");
+        v.do_sample = 1; v.temperature = sp->temperature; v.top_p = sp->top_p; v.top_k = sp->top_k; v.seed = sp->seed;
+    }
+    const int R = lk->num_tokens + 1;
+    std::lock_guard<std::mutex> lk_(m->mu);
+    DeviceGuard dg(m->device);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    // the last step writes rows up to len + (max_new_tokens - 1) + R - 1
+    B2_CHECK_ARG(kv->len_host[0] >= 1 && (int64_t)kv->len_host[0] + lk->max_new_tokens + lk->num_tokens <= kv->max_seq,
+                 "b2_stream_begin_lookup: cache length %d + max_new_tokens %d + num_tokens %d exceed max_seq %d", kv->len_host[0],
+                 lk->max_new_tokens, lk->num_tokens, kv->max_seq);
+    B2_TRY(ws_enter(m, st));
+    B2_TRY(spec_alloc(m, kv, R, st));
+    kv->epoch += 1;
+    v.tag = 1 + kv->epoch % 2047;
+    B2_TRY(set_sampling(kv, v, true, st));
+    B2_CUDA_CHECK(cudaMemsetAsync(kv->step_counter.p, 0, 4, st));
+    B2_TRY(proc_all_off(kv, st));
+    ProcRow off = {};
+    off.penalty = 1.f;
+    B2_TRY(proc_seed(proc_state(kv), 0, off, lk->prompt_ids, lk->prompt_len, -1, m->d.vocab, st));  // the history: prompt ids
+    SpecState ss = {};
+    ss.K = lk->num_tokens; ss.ngram = lk->max_ngram; ss.max_new = lk->max_new_tokens; ss.n_eos = lk->n_eos;
+    for (int i = 0; i < lk->n_eos; ++i) ss.eos[i] = lk->eos_ids[i];
+    ss.prompt_len = lk->prompt_len; ss.hist_len = lk->prompt_len;
+    B2_CUDA_CHECK(cudaHostGetDevicePointer(reinterpret_cast<void**>(&ss.mirror), kv->spec_mirror, 0));
+    B2_CUDA_CHECK(cudaMemcpyAsync(kv->spec_state.p, &ss, sizeof ss, cudaMemcpyHostToDevice, st));
+    B2_CUDA_CHECK(cudaStreamSynchronize(st));  // `ss` is a pageable host source; earlier steps on this cache are done
+    memset(kv->spec_mirror, 0, 6 * sizeof(int));
+    kv->spec_mirror[5] = 1;  // token 0, published below
+    // token 0 from the prefill logits, published as ring entry 0 and pending for the first verify step
+    B2_TRY(sample_publish(logits, m->d.vocab, 1, kv->sstate.as<SampleState>(), kv->rows_dev.as<RowState>(), kv->tok.as<int32_t>(), nullptr,
+                          kv->step_counter.as<int32_t>(), kv->len_dev.as<int32_t>(), kv->ring_dev, kv->ring_cap, SP_SELECT, 0,
+                          proc_state(kv), nullptr, st));
+    kv->stream_B = 1; kv->stream_tag = v.tag; kv->stream_scheduled = 1;
+    kv->spec_R = R; kv->spec_max_new = lk->max_new_tokens; kv->spec_queued = 0; kv->spec_len0 = kv->len_host[0];
+    return ws_leave(m, st);
+}
+
+// b2_stream_enqueue of a lookup generation: tops the verify steps in flight (queued, not yet retired on the device) up to n, and
+// queues none once the generation's tokens are published. A step publishes a varying number of tokens, so steps are scheduled
+// against what the device has retired, read from the mapped mirror without a synchronisation. Every step in flight publishes at
+// least one token until max_new_tokens are out, so the host may wait for token published + in flight - 1.
+static int lookup_enqueue(b2_model* m, b2_kv* kv, int n_steps, cudaStream_t st) {
+    const volatile int* mr = kv->spec_mirror;
+    const int published = mr[5];  // before `retired`: the device writes retired first
+    __sync_synchronize();
+    const int retired = mr[4];
+    int in_flight = kv->spec_queued - retired;
+    if (published < kv->spec_max_new && in_flight < n_steps) {
+        const int q = n_steps - in_flight;
+        B2_TRY(ws_enter(m, st));
+        cudaStream_t run = nullptr;
+        B2_TRY(fork_stream(kv, st, &run));
+        for (int s = 0; s < q; ++s) B2_TRY(verify_step_run(m, kv, kv->spec_R, run));
+        B2_TRY(join_stream(kv, st, run));
+        B2_TRY(ws_leave(m, st));
+        kv->spec_queued += q;
+        in_flight += q;
+        // an upper bound of the cache length (the exact one is in the mirror once the steps have run)
+        kv->len_host[0] = kv->spec_len0 + std::min(kv->spec_max_new - 1, kv->spec_queued * kv->spec_R);
+    }
+    const int guaranteed = published >= kv->spec_max_new ? kv->spec_max_new : std::min(kv->spec_max_new, published + in_flight);
+    kv->stream_scheduled = std::max(kv->stream_scheduled, guaranteed);
+    return 0;
+}
+
+int b2_stream_lookup_stats(b2_kv* kv, int32_t* steps, int32_t* drafted, int32_t* accepted) {
+    B2_CHECK_ARG(kv != nullptr, "b2_stream_lookup_stats: null cache");
+    B2_CHECK_ARG(kv->spec_mirror != nullptr, "b2_stream_lookup_stats: no lookup generation has run on this cache");
+    const volatile int* mr = kv->spec_mirror;
+    if (steps) *steps = mr[0];
+    if (drafted) *drafted = mr[1];
+    if (accepted) *accepted = mr[2];
+    return 0;
+}
+
+int b2_decode_rows(b2_model* m, b2_kv* kv, int slot, const int32_t* tokens, int R, float* logits_out, void* stream) {
+    B2_CHECK_ARG(m && kv && tokens && kv->m == m, "b2_decode_rows: bad handle");
+    B2_CHECK_ARG(m->finalized, "b2_decode_rows: model not finalized");
+    B2_CHECK_ARG(slot >= 0 && slot < kv->max_batch, "b2_decode_rows: slot %d outside the cache's %d", slot, kv->max_batch);
+    std::lock_guard<std::mutex> lk(m->mu);
+    DeviceGuard dg(m->device);
+    B2_CHECK_ARG(kv->len_host[slot] >= 1 && kv->len_host[slot] + R <= kv->max_seq,
+                 "b2_decode_rows: slot %d cache length %d + %d rows exceeds capacity %d (prefill first)", slot, kv->len_host[slot], R,
+                 kv->max_seq);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    B2_TRY(ws_enter(m, st));
+    B2_TRY(spec_alloc(m, kv, R, st));
+    B2_TRY(set_greedy_unpublished(kv, st));
+    B2_CUDA_CHECK(cudaMemcpyAsync(spec_rows(kv), tokens, (size_t)R * 4, cudaMemcpyDefault, st));
+    cudaStream_t run = nullptr;
+    B2_TRY(fork_stream(kv, st, &run));
+    B2_TRY(rows_forward(m, kv, slot, R, run));
+    B2_TRY(join_stream(kv, st, run));
+    const int32_t len = kv->len_host[slot] + R;
+    B2_TRY(set_i32_pairs(kv->len_dev.as<int32_t>() + slot, &len, nullptr, nullptr, 1, st));
+    kv->len_host[slot] = len;
+    if (logits_out)
+        B2_CUDA_CHECK(cudaMemcpyAsync(logits_out, kv->spec_logits.p, (size_t)R * m->d.vocab * 4, cudaMemcpyDefault, st));
+    B2_TRY(ws_leave(m, st));
+    // host sources are copied before return; a host destination must be complete on return
+    if (!is_device_pointer(tokens) || (logits_out && !is_device_pointer(logits_out))) B2_CUDA_CHECK(cudaStreamSynchronize(st));
+    return 0;
+}
+
 int b2_stream_enqueue(b2_model* m, b2_kv* kv, int n_steps, void* stream) {
     B2_CHECK_ARG(m && kv && kv->m == m && n_steps >= 1, "b2_stream_enqueue: bad argument");
     std::lock_guard<std::mutex> lk(m->mu);
     DeviceGuard dg(m->device);
     B2_CHECK_ARG(kv->stream_B >= 1, "b2_stream_enqueue: no streaming generation on this cache (b2_stream_begin first)");
+    if (kv->spec_R > 0) return lookup_enqueue(m, kv, n_steps, reinterpret_cast<cudaStream_t>(stream));
     const int B = kv->stream_B;
     const bool per_row = kv->samp_host.per_row != 0;
     // one generation never outgrows the ring (ring_cap = max_seq); a continuously batched cache runs indefinitely and wraps
@@ -1864,6 +2121,7 @@ int b2_batch_begin(b2_model* m, b2_kv* kv, int B, void* stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     SampleState v = {};
     v.temperature = 1.f; v.top_p = 1.f; v.per_row = 1;
+    kv->spec_R = 0;
     kv->epoch += 1;
     v.tag = 1 + kv->epoch % 2047;
     B2_TRY(ws_enter(m, st));
@@ -2123,6 +2381,69 @@ int b2_op_rope_kv_write(void* qkv, void* kcache, void* vcache, int B, int S, int
                         void* stream) {
     B2_CHECK_ARG(qkv && kcache && vcache, "b2_op_rope_kv_write: null argument");
     return rope_kv_write(qkv, kcache, vcache, B, S, H, D, Smax, theta, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int64_t b2_op_decode_attn_mq_scratch_bytes(int B, int H, int nsplit) {
+    if (B < 1 || H < 1 || nsplit < 1) return -1;
+    return (int64_t)decode_attn_mq_scratch_bytes(B, H, nsplit);
+}
+
+int b2_op_decode_attn_mq_nsplit(int H, int Smax) {
+    B2_CHECK_ARG(H >= 1 && Smax >= 1, "b2_op_decode_attn_mq_nsplit: bad shape");
+    return decode_nsplit(1, H, Smax, decode_attn_mq_ctas_per_sm());
+}
+
+int b2_op_decode_attn_mq(const void* qkv, const void* kcache, const void* vcache, const int32_t* cur_len, void* out, void* scratch,
+                         int B, int R, int H, int Smax, int nsplit, float scale, void* stream) {
+    B2_CHECK_ARG(qkv && kcache && vcache && cur_len && out && scratch, "b2_op_decode_attn_mq: null argument");
+    B2_CHECK_ARG(B >= 1 && H >= 1 && nsplit >= 1 && Smax >= 1, "b2_op_decode_attn_mq: bad shape");
+    DecodeAttnArgs da;
+    da.qkv = qkv; da.kcache = const_cast<void*>(kcache); da.vcache = const_cast<void*>(vcache); da.cur_len = cur_len; da.out = out;
+    da.partial = reinterpret_cast<float*>(scratch);
+    da.counters = reinterpret_cast<int32_t*>(reinterpret_cast<char*>(scratch) + decode_attn_mq_scratch_bytes(B, H, nsplit) -
+                                             (size_t)B * H * sizeof(int32_t));
+    da.B = B; da.R = R; da.H = H; da.D = 128; da.Smax = Smax; da.nsplit = nsplit; da.scale = scale;
+    return decode_attn_mq_bf16(da, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int b2_op_prompt_lookup(const int32_t* hist, int len, int num_tokens, int max_ngram, int max_length, const int32_t* eos_host, int n_eos,
+                        int V, int32_t* out_tokens, int32_t* out_draft_len, void* stream) {
+    B2_CHECK_ARG(hist && out_tokens && out_draft_len && len >= 1, "b2_op_prompt_lookup: bad argument");
+    B2_CHECK_ARG(num_tokens >= 1 && num_tokens < kSpecMaxRows && max_ngram >= 1 && max_length >= 1,
+                 "b2_op_prompt_lookup: num_tokens must be in 1..%d, max_ngram and max_length >= 1", kSpecMaxRows - 1);
+    B2_CHECK_ARG(n_eos >= 0 && n_eos <= kProcMaxEos && (n_eos == 0 || eos_host), "b2_op_prompt_lookup: bad eos ids");
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    // scratch: SpecState, SampleState, tok[1], history [len]
+    const size_t off_st = (sizeof(SpecState) + 255) / 256 * 256, off_tok = off_st + 256, off_hist = off_tok + 256;
+    DevBuf tmp;
+    B2_TRY(tmp.alloc(off_hist + (size_t)len * 4));
+    SpecState ss = {};
+    ss.K = num_tokens; ss.ngram = max_ngram; ss.max_new = max_length; ss.n_eos = n_eos;
+    for (int i = 0; i < n_eos; ++i) ss.eos[i] = eos_host[i];
+    ss.hist_len = len - 1;  // hist[len - 1] is the pending token
+    SampleState sst = {};
+    int32_t* tok = reinterpret_cast<int32_t*>(tmp.as<char>() + off_tok);
+    int32_t* h = reinterpret_cast<int32_t*>(tmp.as<char>() + off_hist);
+    int r = 0;
+    if (cudaMemcpyAsync(tmp.p, &ss, sizeof ss, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemcpyAsync(tmp.as<char>() + off_st, &sst, sizeof sst, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemcpyAsync(h, hist, (size_t)len * 4, cudaMemcpyDefault, st) != cudaSuccess ||
+        cudaMemcpyAsync(tok, hist + len - 1, 4, cudaMemcpyDefault, st) != cudaSuccess) {
+        set_error("b2_op_prompt_lookup: %s", cudaGetErrorString(cudaGetLastError()));
+        r = -2;
+    }
+    SpecState* dss = tmp.as<SpecState>();
+    if (r == 0) r = prompt_lookup(h, dss, reinterpret_cast<SampleState*>(tmp.as<char>() + off_st), tok, V, num_tokens + 1, st);
+    if (r == 0 && (cudaMemcpyAsync(out_tokens, tmp.as<char>() + offsetof(SpecState, rows), (size_t)(num_tokens + 1) * 4, cudaMemcpyDefault, st) != cudaSuccess ||
+                   cudaMemcpyAsync(out_draft_len, tmp.as<char>() + offsetof(SpecState, draft_len), 4, cudaMemcpyDefault, st) != cudaSuccess)) {
+        set_error("b2_op_prompt_lookup: %s", cudaGetErrorString(cudaGetLastError()));
+        r = -2;
+    }
+    cudaError_t e = cudaStreamSynchronize(st);
+    tmp.free();
+    if (r != 0) return r;
+    B2_CUDA_CHECK(e);
+    return 0;
 }
 
 int64_t b2_op_decode_attn_scratch_bytes(int B, int H, int nsplit) {

@@ -171,10 +171,52 @@ __device__ __forceinline__ void process_row(float* s_x, int V, const ProcState& 
     }
 }
 
+// HF 5.5 assisted decoding's acceptance (generation/utils.py, n_matches): the draft's leading tokens that equal the tokens
+// selected at the rows before them are kept, plus the token selected after the last match; a draft that reaches max_length
+// gives up its last match. Runs in the last CTA of the step, after every row's selection is in spec->sel.
+__device__ void spec_accept(SpecState* spec, SampleState* st, int pub, int32_t* tok, int32_t* cur_len, int32_t* hist,
+                            volatile int32_t* ring, int ring_cap) {
+    const int d = spec->draft_len;
+    const volatile int32_t* sel = spec->sel;
+    int n = 0;  // a step queued after the generation published its max_new tokens changes nothing
+    if (pub < spec->max_new) {
+        int m = 0;
+        while (m < d && sel[m] == spec->rows[1 + m]) ++m;
+        const int L = spec->hist_len + 1;  // history length with the pending token
+        if (d > 0 && m == d && L + d >= spec->prompt_len + spec->max_new) m -= 1;  // is_done_candidate
+        n = min(m + 1, spec->max_new - pub);
+        for (int i = 0; i + 1 < n; ++i) hist[L + i] = sel[i];
+        tok[0] = sel[n - 1];
+        spec->hist_len += n;
+        cur_len[0] += n;
+        st->pub_counter = pub + n;
+        spec->steps += 1;
+        spec->drafted += d;
+        spec->accepted += n - 1;
+    }
+    spec->retired += 1;
+    // the mirror before the ring: a host that has read token t finds published > t and the steps retired up to it there
+    if (spec->mirror != nullptr) {
+        volatile int* mr = spec->mirror;
+        mr[0] = spec->steps; mr[1] = spec->drafted; mr[2] = spec->accepted; mr[3] = cur_len[0]; mr[4] = spec->retired;
+        __threadfence_system();
+        mr[5] = pub + n;
+        __threadfence_system();
+    }
+    for (int i = 0; i < n; ++i) {
+        if (ring != nullptr && st->tag != 0) {
+            const int t = pub + i;
+            const int tag = 1 + (st->tag - 1 + t / ring_cap) % 2047;
+            ring[t % ring_cap] = (tag << 20) | (sel[i] & 0xFFFFF);
+        }
+    }
+    __threadfence_system();
+}
+
 __global__ void __launch_bounds__(SP_THREADS, 1)
 sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleState* st, RowState* rows, int32_t* tok, int32_t* out_tokens,
                       int32_t* step_counter, int32_t* cur_len, volatile int32_t* ring, int ring_cap, int flags,
-                      int step_offset, ProcState proc, float* processed_out) {
+                      int step_offset, ProcState proc, float* processed_out, SpecState* spec) {
     extern __shared__ __align__(16) uint8_t sp_smem[];
     float* s_x = reinterpret_cast<float*>(sp_smem);
     __shared__ unsigned long long s_hist[256];
@@ -196,9 +238,13 @@ sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleStat
     const int top_k = per_row ? rows[b].top_k : st->top_k;
     const unsigned long long seed = per_row ? rows[b].seed : st->seed;
     const int pub = st->pub_counter;
-    const int draw = per_row ? rows[b].index : pub;
-    const bool select = active && (flags & SP_SELECT);
-    const bool proc_on = proc.rows != nullptr && proc.rows[b].on != 0 && active;
+    // multi-row acceptance: row b is token pub + b of the generation; rows past the draft (and every row once the generation
+    // has published its max_new tokens) are not selected
+    const int draw = per_row ? rows[b].index : pub + (spec ? b : 0);
+    const uint32_t draw_row = spec ? 0u : (uint32_t)b;
+    const bool spec_idle = spec != nullptr && (b > spec->draft_len || pub >= spec->max_new);
+    const bool select = active && (flags & SP_SELECT) && !spec_idle;
+    const bool proc_on = spec == nullptr && proc.rows != nullptr && proc.rows[b].on != 0 && active;
     int choice = 0;
     const float* row = logits + (size_t)b * V;
     if (select && (proc_on || processed_out != nullptr)) {
@@ -213,6 +259,8 @@ sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleStat
 
     if (!active) {
         choice = tok[b];  // an idle slot keeps its token; nothing is selected or counted for it
+    } else if (spec_idle) {
+        choice = 0;
     } else if (!(flags & SP_SELECT)) {
         choice = tok[b];  // already chosen by the producer of `tok` (decode megakernel's fused argmax)
     } else if (!do_sample) {
@@ -272,7 +320,7 @@ sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleStat
         }
         const unsigned long long excl = warp_base + incl - mine;
         if (tid == 0) {
-            s_target = total ? __umul64hi(total, philox_u64(seed, (uint32_t)draw, (uint32_t)b)) : 0ull;
+            s_target = total ? __umul64hi(total, philox_u64(seed, (uint32_t)draw, draw_row)) : 0ull;
             s_choice = 0;
         }
         __syncthreads();
@@ -291,7 +339,14 @@ sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleStat
         choice = s_choice;
     }
 
-    if (tid == 0) {
+    if (tid == 0 && spec != nullptr) {
+        spec->sel[b] = choice;
+        __threadfence();
+        if (atomicAdd(&st->done, 1u) == (unsigned)B - 1u) {  // last row of the step: accept
+            st->done = 0u;
+            spec_accept(spec, st, pub, tok, cur_len, proc.hist, ring, ring_cap);
+        }
+    } else if (tid == 0) {
         if ((flags & SP_SELECT) && active) tok[b] = choice;
         if (per_row && active) rows[b].index = draw + 1;
         if (proc_on) {  // the chosen token joins the row's history
@@ -320,6 +375,60 @@ sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleStat
                     if (!per_row || rows[i].active) cur_len[i] += 1;
             }
         }
+    }
+}
+
+// HF 5.5 PromptLookupCandidateGenerator.get_candidates over hist[0, L) (the pending token appended at hist_len): n-gram sizes
+// min(ngram, L - 1) .. 1; for each, the leftmost earlier occurrence of the last n ids with a continuation wins; the draft is
+// hist[start, min(start + K, L, max_length)), cut before the first eos id and (unlike HF, which would feed the -200 image
+// placeholder to the model) before the first id outside [0, V)
+constexpr int LK_THREADS = 256;
+__global__ void __launch_bounds__(LK_THREADS)
+prompt_lookup_kernel(int32_t* hist, SpecState* spec, const SampleState* st, const int32_t* tok, int V, int R) {
+    __shared__ int s_start;
+    const int tid = threadIdx.x;
+    pdl_trigger();
+    pdl_wait();  // tok, the history and the counters are written by the previous step's acceptance
+    const int h0 = spec->hist_len, K = spec->K;
+    const int L = h0 + 1;
+    const int pending = tok[0];
+    const int max_length = spec->prompt_len + spec->max_new;
+    if (tid == 0) hist[h0] = pending;
+    __syncthreads();
+    int start = -1, end = -1;
+    if (st->pub_counter < spec->max_new && max_length != L + 1) {
+        const int lim = min(L, max_length);  // a match must start its continuation before lim
+        for (int n = min(spec->ngram, L - 1); n >= 1; --n) {
+            if (tid == 0) s_start = INT_MAX;
+            __syncthreads();
+            const int32_t* tail = hist + (L - n);
+            for (int s = tid; s + n < lim; s += LK_THREADS) {
+                bool match = true;
+                for (int i = 0; i < n && match; ++i) match = hist[s + i] == tail[i];
+                if (match) atomicMin(&s_start, s);
+            }
+            __syncthreads();
+            const int s0 = s_start;
+            __syncthreads();
+            if (s0 != INT_MAX) {
+                start = s0 + n;
+                end = min(start + K, lim);
+                break;
+            }
+        }
+    }
+    if (tid == 0) {
+        int d = 0;
+        for (int i = start; start >= 0 && i < end; ++i) {
+            const int id = hist[i];
+            bool stop = id < 0 || id >= V;
+            for (int e = 0; e < spec->n_eos; ++e) stop = stop || id == spec->eos[e];
+            if (stop) break;
+            spec->rows[1 + d++] = id;
+        }
+        spec->rows[0] = pending;
+        for (int j = 1 + d; j < R; ++j) spec->rows[j] = pending;
+        spec->draft_len = d;
     }
 }
 
@@ -374,10 +483,20 @@ int proc_seed(const ProcState& proc, int row, const ProcRow& v, const int64_t* i
     return 0;
 }
 
+int prompt_lookup(int32_t* hist, SpecState* spec, const SampleState* st, const int32_t* tok, int V, int R, cudaStream_t stream) {
+    B2_CHECK_ARG(hist != nullptr && spec != nullptr && st != nullptr && tok != nullptr && R >= 2 && R <= kSpecMaxRows,
+                 "prompt_lookup: bad argument");
+    B2_CUDA_CHECK(launch_pdl(prompt_lookup_kernel, dim3(1), dim3(LK_THREADS), 0, stream, hist, spec, st, tok, V, R));
+    B2_LAUNCH_CHECK();
+    return 0;
+}
+
 int sample_publish(const float* logits, int V, int B, SampleState* st_dev, RowState* rows_dev, int32_t* tok, int32_t* out_tokens,
                    int32_t* step_counter, int32_t* cur_len, int32_t* ring_dev, int ring_cap, int flags, int step_offset,
-                   const ProcState& proc, float* processed_out, cudaStream_t stream) {
+                   const ProcState& proc, float* processed_out, cudaStream_t stream, SpecState* spec) {
     B2_CHECK_ARG(B >= 1 && V >= 1 && st_dev != nullptr && tok != nullptr, "sample_publish: bad argument");
+    B2_CHECK_ARG(spec == nullptr || (B <= kSpecMaxRows && flags == SP_SELECT && proc.hist != nullptr && rows_dev == nullptr),
+                 "sample_publish: bad multi-row acceptance");
     B2_CHECK_ARG(V < (1 << 20), "sample_publish: vocab %d does not fit the 20-bit token field of the host ring", V);
     const size_t smem = sample_smem_bytes(V);
     B2_CHECK_ARG(smem <= 200 * 1024, "sample_publish: vocab %d exceeds the shared-memory staging of the sampling kernel", V);
@@ -387,7 +506,7 @@ int sample_publish(const float* logits, int V, int B, SampleState* st_dev, RowSt
         attr = smem;
     }
     B2_CUDA_CHECK(launch_pdl(sample_publish_kernel, dim3(B), dim3(SP_THREADS), smem, stream, logits, V, B, st_dev, rows_dev, tok,
-                             out_tokens, step_counter, cur_len, ring_dev, ring_cap, flags, step_offset, proc, processed_out));
+                             out_tokens, step_counter, cur_len, ring_dev, ring_cap, flags, step_offset, proc, processed_out, spec));
     B2_LAUNCH_CHECK();
     return 0;
 }

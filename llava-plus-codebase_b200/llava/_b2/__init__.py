@@ -71,6 +71,29 @@ class LogitsProc(_c.Structure):
 MAX_PROC_EOS = 8
 
 
+class PromptLookup(_c.Structure):
+    """b2_prompt_lookup (include/b2llava.h): prompt-lookup speculative decoding of one sample; `prompt_ids` is a device int64
+    pointer."""
+    _fields_ = [("num_tokens", _c.c_int32), ("max_ngram", _c.c_int32), ("max_new_tokens", _c.c_int32), ("n_eos", _c.c_int32),
+                ("eos_ids", _c.c_int32 * 8), ("prompt_ids", _vp), ("prompt_len", _c.c_int32)]
+
+
+def make_prompt_lookup(prompt_row, num_tokens, max_ngram, max_new_tokens, eos_ids=()):
+    """PromptLookup over `prompt_row` (device int64 [L], kept alive as `.ids` of the result)."""
+    eos = sorted(set(int(e) for e in eos_ids))
+    if len(eos) > MAX_PROC_EOS:
+        raise ValueError(f"at most {MAX_PROC_EOS} eos ids are supported with prompt lookup, got {len(eos)}")
+    if prompt_row.dtype != torch.int64 or prompt_row.dim() != 1 or not prompt_row.is_cuda or not prompt_row.is_contiguous():
+        raise ValueError("prompt_row must be a contiguous 1-D int64 CUDA tensor")
+    lk = PromptLookup(int(num_tokens), int(max_ngram), int(max_new_tokens), len(eos))
+    for i, e in enumerate(eos):
+        lk.eos_ids[i] = e
+    lk.prompt_ids = prompt_row.data_ptr() if prompt_row.numel() else None
+    lk.prompt_len = int(prompt_row.numel())
+    lk.ids = prompt_row
+    return lk
+
+
 def make_logits_proc(prompt_row, repetition_penalty=1.0, no_repeat_ngram_size=0, min_generated=0, eos_ids=()):
     """LogitsProc over `prompt_row` (device int64 [L], kept alive as `.ids` of the result; a caller that hands the struct to
     work on another stream records that stream on it), or None when every processor is at its off value. min_generated: eos ids are banned while fewer tokens were generated."""
@@ -140,6 +163,9 @@ SIGNATURES = {
     "b2_stream_begin_ex": (_i32, [_vp, _vp, _vp, _i32, _c.POINTER(Sampling), _c.POINTER(LogitsProc), _vp]),
     "b2_stream_enqueue": (_i32, [_vp, _vp, _i32, _vp]),
     "b2_stream_wait": (_i32, [_vp, _i32, _c.POINTER(_c.c_int32), _i32]),
+    "b2_stream_begin_lookup": (_i32, [_vp, _vp, _vp, _i32, _c.POINTER(Sampling), _c.POINTER(PromptLookup), _vp]),
+    "b2_stream_lookup_stats": (_i32, [_vp, _c.POINTER(_c.c_int32), _c.POINTER(_c.c_int32), _c.POINTER(_c.c_int32)]),
+    "b2_decode_rows": (_i32, [_vp, _vp, _i32, _vp, _i32, _vp, _vp]),
     "b2_op_preprocess_clip": (_i32, [_c.POINTER(PreprocessPlan), _vp]),
     "b2_op_sample": (_i32, [_vp, _i32, _i32, _c.POINTER(Sampling), _i32, _vp, _vp]),
     "b2_op_sample_ex": (_i32, [_vp, _i32, _i32, _c.POINTER(Sampling), _c.POINTER(LogitsProc), _i32, _vp, _vp, _vp]),
@@ -176,6 +202,10 @@ SIGNATURES = {
     "b2_op_decode_attn_scratch_bytes": (_i64, [_i32, _i32, _i32]),
     "b2_op_decode_attn_e4m3": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _f32, _vp]),
     "b2_op_decode_attn_nsplit": (_i32, [_i32, _i32, _i32, _i32]),
+    "b2_op_decode_attn_mq": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp]),
+    "b2_op_decode_attn_mq_scratch_bytes": (_i64, [_i32, _i32, _i32]),
+    "b2_op_decode_attn_mq_nsplit": (_i32, [_i32, _i32]),
+    "b2_op_prompt_lookup": (_i32, [_vp, _i32, _i32, _i32, _i32, _c.POINTER(_c.c_int32), _i32, _i32, _vp, _vp, _vp]),
     "b2_op_kv_quantize_e4m3": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
     "b2_op_kv_quantize_e4m3_at": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
     "b2_op_kv_dequantize_e4m3": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
@@ -482,6 +512,32 @@ class Engine:
             else:
                 check(self.lib.b2_stream_begin_ex(self.handle, kv.handle, ptr(logits), B, ctypes.byref(sp), arr, stream_ptr()),
                       "b2_stream_begin_ex")
+
+    def stream_begin_lookup(self, kv, logits, sampling, lookup):
+        """stream_begin of a batch-1 prompt-lookup generation (`lookup`: make_prompt_lookup); stream_enqueue(n) then queues n
+        verify steps, each publishing at least one token."""
+        logits = logits.contiguous()
+        sp = sampling if sampling is not None else make_sampling()
+        with torch.cuda.device(self.index):
+            check(self.lib.b2_stream_begin_lookup(self.handle, kv.handle, ptr(logits), int(logits.shape[0]), ctypes.byref(sp),
+                                                  ctypes.byref(lookup), stream_ptr()), "b2_stream_begin_lookup")
+
+    def lookup_stats(self, kv):
+        """(verify steps, drafted tokens, accepted draft tokens) of the cache's last lookup generation; waits for its steps."""
+        out = [_c.c_int32(0) for _ in range(3)]
+        with torch.cuda.device(self.index):
+            check(self.lib.b2_stream_lookup_stats(kv.handle, *[ctypes.byref(o) for o in out]), "b2_stream_lookup_stats")
+        return tuple(int(o.value) for o in out)
+
+    def decode_rows(self, kv, tokens, slot=0):
+        """The verify forward: tokens int [R] appended at slot `slot`'s length; returns fp32 logits [R, vocab] (device)."""
+        tokens = torch.as_tensor(tokens).to(device=self.device, dtype=torch.int32).contiguous()
+        R = tokens.numel()
+        logits = torch.empty(R, self.vocab, dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.index):
+            check(self.lib.b2_decode_rows(self.handle, kv.handle, int(slot), ptr(tokens), R, ptr(logits), stream_ptr()),
+                  "b2_decode_rows")
+        return logits
 
     def batch_begin(self, kv, B):
         with torch.cuda.device(self.index):

@@ -26,6 +26,7 @@ from transformers.modeling_outputs import CausalLMOutputWithPast
 from ..llava_arch import LlavaMetaModel, LlavaMetaForCausalLM
 from ..multimodal_encoder.clip_encoder import _Holder, _read_checkpoint_dir
 from ..._b2 import (Engine, KVCache, LOGITS_ALL, LOGITS_LAST, ERR_SPLICE_SLOTS, INT32_MIN, kv_dtype_code, last_error, make_logits_proc,
+                     make_prompt_lookup,
                     make_sampling)
 from ..._b2 import prefix as _prefix
 from ...constants import IMAGE_TOKEN_INDEX
@@ -515,6 +516,8 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                                              kwargs)
         if return_dict_in_generate or output_scores:
             raise NotImplementedError("generate() returns the id tensor only")
+        prompt = inputs if inputs.dim() == 2 else inputs.unsqueeze(0)
+        lookup_args = self._prompt_lookup_arguments(kwargs, prompt.shape[0], num_beams, bool(proc_args))
         for k, v in kwargs.items():
             if k in self._IGNORED_GENERATION_ARGS:
                 continue
@@ -523,7 +526,6 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                     continue
                 raise NotImplementedError(f"generate({k}={v!r}) is not implemented on the H100 path")
             raise NotImplementedError(f"generate() got an unsupported argument {k!r}")
-        prompt = inputs if inputs.dim() == 2 else inputs.unsqueeze(0)
         B, Lt = prompt.shape
         engine = self._ensure_engine()
         if eos_token_id is None:
@@ -557,6 +559,11 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                      for b in range(B)]
             if all(p is None for p in procs):
                 procs = None
+        lookup = None  # prompt-lookup speculative decoding (batch 1): lookup(cache rows) -> PromptLookup, or None when K rows no longer fit
+        if lookup_args and self._get_batcher(engine) is None:
+            def lookup(rows):
+                return self._fit_prompt_lookup(engine, prompt, rows, lookup_args, max_new_tokens, eos_ids)
+        began_lookup = [False]
         prof = _StageTimer() if os.environ.get("B2_PROFILE_GENERATE") else None
 
         batcher = self._get_batcher(engine) if B == 1 else None
@@ -606,13 +613,18 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 self._check_limits(engine, B, max(lens) + max_new_tokens)
                 kv.reset()
                 logits = engine.prefill(kv, embeds, lens, LOGITS_LAST)
-                engine.stream_begin(kv, logits, sampling, procs)
+                lk = lookup(lens[0]) if lookup is not None else None
+                began_lookup[0] = lk is not None
+                if lk is not None:
+                    engine.stream_begin_lookup(kv, logits, sampling, lk)
+                else:
+                    engine.stream_begin(kv, logits, sampling, procs)
                 engine.stream_wait(kv, 0, B)          # first sync of this call: every input check has run by now
                 if prof: prof.mark("prefill + first token")
                 return speculative
 
             if plan is not None:
-                self._prefill_reusing(engine, kv, plan, reuse, released_ev, sampling, max_new_tokens, procs)
+                began_lookup[0] = self._prefill_reusing(engine, kv, plan, reuse, released_ev, sampling, max_new_tokens, procs, lookup)
                 speculative = False
             else:
                 speculative = prefill(False)
@@ -630,7 +642,8 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             pad = pad_token_id if pad_token_id is not None else (next(iter(eos_ids)) if eos_ids else 0)
             new_tokens = _stream_decode(engine, kv, None, sampling, B, max_new_tokens, eos_ids, pad, prompt,
                                         streamer, stopping_criteria,
-                                        run_ahead=int(getattr(self.config, "b2_run_ahead", 8)), begun=True)
+                                        run_ahead=int(getattr(self.config, "b2_run_ahead", 8)), begun=True,
+                                        lookup_steps=_LOOKUP_STEPS_IN_FLIGHT if began_lookup[0] else 0)
             engine.check_async_error()
             if prof: prof.mark("decode")
             if plan is not None:
@@ -688,6 +701,65 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         if p == 1.0 and n == 0 and mnt <= 0 and ml <= 0:
             return {}
         return {"repetition_penalty": p, "no_repeat_ngram_size": n, "min_new_tokens": mnt, "min_length": ml}
+
+    # ------------------------------------------------------------------ prompt-lookup speculative decoding
+    def _prompt_lookup_cap(self):
+        """config.b2_prompt_lookup or B2_PROMPT_LOOKUP: K, the most draft tokens per verify step (0 = off). It caps
+        prompt_lookup_num_tokens, and batch-1 calls that do not pass it draft K tokens."""
+        v = getattr(self.config, "b2_prompt_lookup", None)
+        if v is None:
+            v = os.environ.get("B2_PROMPT_LOOKUP")
+        try:
+            k = int(v or 0)
+        except (TypeError, ValueError):
+            raise ValueError(f"b2_prompt_lookup must be an integer, got {v!r}")
+        if not 0 <= k <= 15:
+            raise ValueError(f"b2_prompt_lookup must be in 0..15, got {k}")
+        return k
+
+    def _fit_prompt_lookup(self, engine, prompt, rows, lookup_args, max_new_tokens, eos_ids):
+        """The PromptLookup of a batch-1 generation whose prompt fills `rows` cache rows. A verify step writes K rows past the
+        last token, so K is capped at what the cache leaves free; with no room (or more eos ids than the device keeps) the
+        call decodes without speculation, as it would without the opt-in."""
+        Lt = prompt.shape[1]
+        room = self._pool.max_seq - max(rows, Lt) - max_new_tokens
+        k = min(lookup_args["num_tokens"], room)
+        if getattr(self.config, "b2_fp8_decode", False) or os.environ.get("B2_FP8_DECODE") == "1":
+            k = min(k, engine.desc.max_batch - 1)  # the e4m3 activation buffer holds max_batch rows
+        if k < 1 or len(set(eos_ids)) > 8:
+            return None
+        prompt_dev = prompt.to(device=engine.device, dtype=torch.int64).contiguous()
+        return make_prompt_lookup(prompt_dev[0], k, lookup_args["max_ngram"], max_new_tokens, eos_ids)
+
+    def _prompt_lookup_arguments(self, kwargs, B, num_beams, has_procs):
+        """With the opt-in, takes prompt_lookup_num_tokens / max_matching_ngram_size out of `kwargs` and returns
+        {"num_tokens", "max_ngram"} when this call decodes with prompt lookup, else {}. Without it they stay in `kwargs` and raise
+        as any unsupported argument does."""
+        K = self._prompt_lookup_cap()
+        if K == 0:
+            return {}
+        k = kwargs.pop("prompt_lookup_num_tokens", None)
+        n = kwargs.pop("max_matching_ngram_size", None)
+        explicit = k is not None
+        if explicit:
+            k = int(k)
+            if k <= 0:
+                raise ValueError("Invalid max_matching_ngram_size or num_output_tokens")
+            if B != 1:
+                raise ValueError("assisted generate is only supported for batch_size = 1")
+            blocker = ("the continuous batcher (b2_continuous_batching)" if int(getattr(self.config, "b2_continuous_batching", 0) or 0)
+                       else "num_beams > 1" if num_beams != 1 else "logits processors" if has_procs
+                       else "an e4m3 KV cache" if (getattr(self.config, "b2_kv_dtype", None) or os.environ.get("B2_KV_DTYPE") or "bf16") != "bf16"
+                       else None)
+            if blocker is not None:
+                raise NotImplementedError(f"prompt_lookup_num_tokens together with {blocker} is not implemented on the H100 path")
+        elif (B != 1 or num_beams != 1 or has_procs
+              or (getattr(self.config, "b2_kv_dtype", None) or os.environ.get("B2_KV_DTYPE") or "bf16") != "bf16"):
+            return {}
+        n = 2 if n is None else int(n)
+        if n <= 0:
+            raise ValueError("Invalid max_matching_ngram_size or num_output_tokens")
+        return {"num_tokens": min(k, K) if explicit else K, "max_ngram": n}
 
     # ------------------------------------------------------------------ beam search
     def _beam_search_cap(self):
@@ -796,10 +868,11 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             return None
         return {"items": items, "slots": slots, "images": images}
 
-    def _prefill_reusing(self, engine, kv, plan, m, released_ev, sampling, max_new_tokens, procs=None):
+    def _prefill_reusing(self, engine, kv, plan, m, released_ev, sampling, max_new_tokens, procs=None, lookup=None):
         """Prefill of a planned prompt that keeps the first m spliced rows of `kv`: image slots wholly inside them are not
         encoded, rows [m, L) are spliced on the host-index path and prefilled at position m (b2_prefill_at). m == 0 is an
-        ordinary prefill from position 0. Chooses and publishes token 0 like generate()'s own prefill."""
+        ordinary prefill from position 0. Chooses and publishes token 0 like generate()'s own prefill. Returns whether the
+        generation decodes with prompt lookup (`lookup`: generate()'s lookup(rows) or None)."""
         P = engine.num_patches
         items, slots = plan["items"], plan["slots"]
         rows = [_prefix.item_rows(x, P) for x in slots]
@@ -832,8 +905,13 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         else:
             kv.reset()
             logits = engine.prefill(kv, embeds, None, LOGITS_LAST)
-        engine.stream_begin(kv, logits, sampling, procs)
+        lk = lookup(L) if lookup is not None else None
+        if lk is not None:
+            engine.stream_begin_lookup(kv, logits, sampling, lk)
+        else:
+            engine.stream_begin(kv, logits, sampling, procs)
         engine.stream_wait(kv, 0, 1)
+        return lk is not None
 
     # ------------------------------------------------------------------ checkpoints
     @classmethod
@@ -904,13 +982,21 @@ def _check_weight_format(config):
     return fmt
 
 
+# verify steps a prompt-lookup generation keeps queued in front of the host: two keep the device busy while the host handles a
+# step's tokens, and bound what runs after the host stops
+_LOOKUP_STEPS_IN_FLIGHT = 2
+
+
 def _stream_decode(engine, kv, logits, sampling, B, max_new_tokens, eos_ids, pad, prompt, streamer, stopping_criteria,
-                   run_ahead=8, begun=False):
+                   run_ahead=8, begun=False, lookup_steps=0):
     """Host half of the decode loop. The device chooses token 0 from the prefill `logits` and then runs up to `run_ahead`
     steps in front of this loop; `engine.stream_wait(kv, t, B)` hands over token t as soon as its kernel has written it
     to pinned memory. Per token, in the order HF's loop uses: finished rows show `pad`; streamer.put; eos bookkeeping;
     stopping criteria on cat(prompt, tokens so far) (the reference's KeywordsStoppingCriteria looks at the tail of that
-    tensor, llava/mm_utils.py:92-114). Returns a CPU int64 tensor [B, n], 1 <= n <= max_new_tokens."""
+    tensor, llava/mm_utils.py:92-114). Returns a CPU int64 tensor [B, n], 1 <= n <= max_new_tokens.
+    lookup_steps > 0 (a prompt-lookup generation): a step publishes a varying number of tokens, so instead of counting tokens the
+    loop asks the engine before each token to keep `lookup_steps` verify steps in flight (b2_stream_enqueue tops them up against
+    the steps the device has retired and queues none once max_new_tokens are published)."""
     Lt = prompt.shape[1]
     crit_buf = None
     if stopping_criteria:
@@ -923,8 +1009,10 @@ def _stream_decode(engine, kv, logits, sampling, B, max_new_tokens, eos_ids, pad
     finished = [False] * B
     cols = []
     for t in range(max_new_tokens):
+        if lookup_steps > 0:
+            engine.stream_enqueue(kv, lookup_steps)
         # keep the device `run_ahead` tokens in front of the host (queued in blocks: one call per ~run_ahead/2 tokens)
-        if scheduled < max_new_tokens and scheduled - t <= (run_ahead + 1) // 2:
+        elif scheduled < max_new_tokens and scheduled - t <= (run_ahead + 1) // 2:
             n = min(run_ahead - (scheduled - t) + 1, max_new_tokens - scheduled)
             if n > 0:
                 engine.stream_enqueue(kv, n)
