@@ -317,6 +317,32 @@ int b2_op_beam_topk(const float* logits, const int32_t* row_of_beam, const float
                     float* out_scores, int32_t* out_tokens, int32_t* out_beams, void* stream);
 int b2_beam_step(b2_model* m, b2_kv* kv, const b2_beam_step_args* args, void* stream);
 
+/* Beam sampling (generate(do_sample=True, num_beams > 1): HF 5.5 _beam_search with do_sample). The candidates of a sample are
+ * drawn without replacement instead of taken best first:
+ *   b2_op_beam_sample  per beam row, w = log_softmax(logits[row_of_beam[b*nb + j]]) / temperature (fp32: ((x - max) - lse) / T),
+ *                      then top-k (ties kept) and top-p over w, each keeping at least min_keep tokens, the others -inf; the
+ *                      accumulated score acc = w + beam_scores[b*nb + j]; every finite acc gets the key fp32(acc + g) with
+ *                      g = -log(-log u) in fp64 and u = ((r >> 11) + 0.5) * 2^-53, r = Philox4x32-10(seed; step,
+ *                      (b*nb + j) * V + token). Per sample the K largest keys are returned in key order, each with its
+ *                      unperturbed acc as the score: torch.multinomial(softmax(acc), K) in distribution and in draw order.
+ *                      -inf candidates rank below every finite key by lower beam * V + token, NaN logits below them
+ *                      (a NaN logit stays NaN through the warpers, score NaN).
+ *                      Arguments as b2_op_beam_topk, plus temperature > 0, top_k >= 0 (0 = off), top_p in (0, 1] (1 = off),
+ *                      1 <= min_keep <= K, B * nb * V <= 2^32.
+ *   b2_beam_step_ex    b2_beam_step whose candidates come from b2_op_beam_sample at `step` (NULL sampling = b2_beam_step). */
+typedef struct b2_beam_sampling {
+    float temperature;
+    int32_t top_k;
+    float top_p;
+    int32_t min_keep;         /* HF: 1 + number of eos ids, 2 when there are none */
+    unsigned long long seed;
+} b2_beam_sampling;
+int b2_op_beam_sample(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
+                      const b2_beam_sampling* sampling, uint32_t step, float* out_scores, int32_t* out_tokens, int32_t* out_beams,
+                      void* stream);
+int b2_beam_step_ex(b2_model* m, b2_kv* kv, const b2_beam_step_args* args, const b2_beam_sampling* sampling, uint32_t step,
+                    void* stream);
+
 /* ---- single-kernel entry points (unit-level parity tests; same kernels the hot path launches) ----------- */
 int b2_op_gemm(const void* A, int lda, const void* W, int ldw, const void* bias, const void* residual, int ld_res,
                void* out, int ld_out, int out_fp32, int M, int N, int K, int act, int bn_override, void* stream);

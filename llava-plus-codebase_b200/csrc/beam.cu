@@ -7,6 +7,12 @@
 //     memory, turns it into scores in place, radix-selects the row's K-th best key and compacts the row's top K in index
 //     order; a second launch merges the nb sorted lists of each sample by rank (binary search in every list).
 //     A candidate is one 64-bit key: order_key(score) << 32 | ~flat, so "larger key" is exactly the ranking rule above.
+//   * beam_sample (generate(do_sample=True, num_beams > 1)): the same two launches, but the row kernel warps the log-softmax
+//     row (temperature, top-k, top-p with at least min_keep survivors, HF 5.5's warpers on log-probabilities) and ranks each
+//     finite survivor by the Gumbel-perturbed key fp32(acc + g), g = -log(-log u), u from Philox(seed; step, global flat index).
+//     The K largest keys in order are HF's torch.multinomial(softmax(acc), K) draw order (multinomial without replacement is
+//     top-K of p / Exp(1) there). Warped-away tokens (-inf) rank below every finite key by index, NaN logits below those. The
+//     merge carries each candidate's unperturbed score acc beside its key.
 //   * kv_copy_slots: cache slot dst := rows [row_begin, end) of slot src for every layer, head, K and V (and the fp32 scale
 //     rows of an e4m3 cache); one (layer, head, K|V) slab of one slot is contiguous, so each CTA streams 64 rows with
 //     16-byte vectors. The caller guarantees that no dst is also a src (b2_kv_copy_slots checks it), so pairs are independent.
@@ -15,6 +21,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "select.cuh"
 
 namespace b2 {
 namespace {
@@ -49,119 +56,205 @@ __device__ __forceinline__ float block_reduce(float v, float* s_w, int tid) {
     return t;
 }
 
-__global__ void __launch_bounds__(BT_THREADS, 1)
-beam_row_topk_kernel(const float* __restrict__ logits, const int32_t* __restrict__ row_of_beam, const float* __restrict__ beam_scores,
-                     int nb, int V, int K, unsigned long long* __restrict__ keys_out) {
-    extern __shared__ __align__(16) uint8_t bt_smem[];
-    float* s_x = reinterpret_cast<float*>(bt_smem);
-    __shared__ float s_w[BT_THREADS / 32];
-    __shared__ int s_wa[BT_THREADS / 32];
-    __shared__ int s_gt;
-    __shared__ unsigned int s_hist[256];
-    __shared__ uint32_t s_prefix;
-    __shared__ int s_above;
-    __shared__ unsigned long long s_cand[128];
+// Shared state of one row CTA's candidate selection
+struct RowSmem {
+    float w[BT_THREADS / 32];
+    int wa[BT_THREADS / 32];
+    unsigned long long wsum[BT_THREADS / 32];
+    unsigned long long hist[256];
+    unsigned long long above;
+    uint32_t prefix;
+    int gt;
+    unsigned long long cand[128];
+};
 
-    const int tid = threadIdx.x, j = blockIdx.x, b = blockIdx.y;
-    const int beam = b * nb + j;
-    const int row = row_of_beam ? row_of_beam[beam] : beam;
-    const float* x = logits + (size_t)row * V;
-    const int Kr = K < V ? K : V;  // candidates this row can supply
-
-    float mx = -INFINITY;
-    for (int i = tid; i < V; i += BT_THREADS) {
-        const float v = x[i];
-        s_x[i] = v;
-        if (v > mx) mx = v;  // NaN never compares greater
-    }
-    mx = block_reduce<true>(mx, s_w, tid);
-    float part = 0.f;
-    for (int i = tid; i < V; i += BT_THREADS) {
-        const float v = s_x[i];
-        if (v == v) part += expf(v - mx);
-    }
-    const float lse = logf(block_reduce<false>(part, s_w, tid));
-    const float run = beam_scores[beam];
-    for (int i = tid; i < V; i += BT_THREADS) s_x[i] = ((s_x[i] - mx) - lse) + run;
-    __syncthreads();
-
-    // radix descent for the key of the Kr-th largest score (8 bits per level from the top)
-    if (tid == 0) { s_prefix = 0u; s_above = 0; }
-    for (int level = 0; level < 4; ++level) {
-        const int shift = 24 - 8 * level;
-        if (tid < 256) s_hist[tid] = 0u;
-        __syncthreads();
-        const uint32_t prefix = s_prefix;
-        // log-probabilities crowd into a few digits (at level 0 nearly all share sign and exponent): one shared atomic per
-        // distinct digit of a warp instead of one per element, or the adds to the crowded bin serialise
-        for (int base = 0; base < V; base += BT_THREADS) {
-            const int i = base + tid;
-            const uint32_t key = i < V ? order_key(s_x[i]) : 0u;
-            const bool take = i < V && (level == 0 || (key >> (shift + 8)) == prefix);
-            const uint32_t digit = take ? ((key >> shift) & 255u) : 256u;
-            const unsigned peers = __match_any_sync(0xffffffffu, digit);
-            if (take && (tid & 31) == __ffs(peers) - 1) atomicAdd(&s_hist[digit], (unsigned)__popc(peers));
-        }
-        __syncthreads();
-        if (tid == 0) {
-            int acc = s_above, pick = 0;
-            for (int d = 255; d >= 0; --d) {
-                if (acc + (int)s_hist[d] >= Kr) { pick = d; break; }
-                acc += (int)s_hist[d];
-            }
-            s_above = acc;
-            s_prefix = (prefix << 8) | (uint32_t)pick;
-        }
-        __syncthreads();
-    }
-    const uint32_t kth = s_prefix;
-
-    // compaction in index order, 1024 consecutive elements per pass (a warp reads 32 consecutive words: no bank conflicts):
-    // every element above kth (their order does not matter, the rank sort below orders them), then the lowest-index elements
-    // equal to kth until Kr are taken. s_above now counts the elements above kth.
-    const int n_gt = s_above, need_eq = Kr - n_gt;
-    const unsigned long long flat0 = (unsigned long long)j * V;
+// The row's Kr best 64-bit candidates order_key(s_x[i]) << 32 | ~(flat0 + i) into sm.cand[0, Kr), unordered: a radix select
+// of the Kr-th largest key, then compaction in index order, 1024 consecutive elements per pass (a warp reads 32 consecutive
+// words: no bank conflicts): every element above the Kr-th key, then the lowest-index elements equal to it until Kr are taken.
+__device__ __forceinline__ void row_top_candidates(const float* s_x, int V, int Kr, unsigned long long flat0, int tid, RowSmem& sm) {
+    const uint32_t kth = radix_select<BT_THREADS, false>(
+        V, (unsigned long long)Kr, tid, [&](int i) { return order_key(s_x[i]); }, [](int) { return 1ull; }, sm.hist, &sm.prefix,
+        &sm.above);
+    const int n_gt = (int)sm.above, need_eq = Kr - n_gt;
     const int lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) s_gt = 0;
+    if (tid == 0) sm.gt = 0;
     __syncthreads();
     int eq_seen = 0;  // uniform: elements equal to kth in the passes before this one
     for (int base = 0; base < V; base += BT_THREADS) {
         const int i = base + tid;
         const uint32_t key = i < V ? order_key(s_x[i]) : 0u;
         const unsigned long long cand = ((unsigned long long)key << 32) | (uint32_t)(0xFFFFFFFFu - (uint32_t)(flat0 + i));
-        if (i < V && key > kth) s_cand[atomicAdd(&s_gt, 1)] = cand;
+        if (i < V && key > kth) sm.cand[atomicAdd(&sm.gt, 1)] = cand;
         const bool eq = i < V && key == kth;
         const unsigned bal = __ballot_sync(0xffffffffu, eq);
-        if (lane == 0) s_wa[warp] = __popc(bal);
+        if (lane == 0) sm.wa[warp] = __popc(bal);
         __syncthreads();
         int before = 0, total = 0;
         for (int w = 0; w < BT_THREADS / 32; ++w) {
-            before += w < warp ? s_wa[w] : 0;
-            total += s_wa[w];
+            before += w < warp ? sm.wa[w] : 0;
+            total += sm.wa[w];
         }
         if (eq) {
             const int r = eq_seen + before + __popc(bal & ((1u << lane) - 1u));
-            if (r < need_eq) s_cand[n_gt + r] = cand;
+            if (r < need_eq) sm.cand[n_gt + r] = cand;
         }
         eq_seen += total;
+        // sm.gt is final for this pass after the barrier above; read it before the next one, after which a faster warp may
+        // already add to it in the next pass, so that every thread tests the same value
+        const int gt = sm.gt;
         __syncthreads();
-        if (eq_seen >= need_eq && s_gt == n_gt) break;  // uniform: both parts complete
+        if (eq_seen >= need_eq && gt == n_gt) break;  // uniform: both parts complete
     }
+    __syncthreads();
+}
+
+// Stages logits row `row` in s_x and returns its max (NaN skipped) and log-sum-exp: torch's log_softmax is (x - mx) - lse
+__device__ __forceinline__ void stage_row(const float* __restrict__ x, float* s_x, int V, int tid, RowSmem& sm, float& mx, float& lse) {
+    mx = -INFINITY;
+    for (int i = tid; i < V; i += BT_THREADS) {
+        const float v = x[i];
+        s_x[i] = v;
+        if (v > mx) mx = v;  // NaN never compares greater
+    }
+    mx = block_reduce<true>(mx, sm.w, tid);
+    float part = 0.f;
+    for (int i = tid; i < V; i += BT_THREADS) {
+        const float v = s_x[i];
+        if (v == v) part += expf(v - mx);
+    }
+    lse = logf(block_reduce<false>(part, sm.w, tid));
+}
+
+__global__ void __launch_bounds__(BT_THREADS, 1)
+beam_row_topk_kernel(const float* __restrict__ logits, const int32_t* __restrict__ row_of_beam, const float* __restrict__ beam_scores,
+                     int nb, int V, int K, unsigned long long* __restrict__ keys_out) {
+    extern __shared__ __align__(16) uint8_t bt_smem[];
+    float* s_x = reinterpret_cast<float*>(bt_smem);
+    __shared__ RowSmem sm;
+
+    const int tid = threadIdx.x, j = blockIdx.x, b = blockIdx.y;
+    const int beam = b * nb + j;
+    const int row = row_of_beam ? row_of_beam[beam] : beam;
+    const int Kr = K < V ? K : V;  // candidates this row can supply
+
+    float mx, lse;
+    stage_row(logits + (size_t)row * V, s_x, V, tid, sm, mx, lse);
+    const float run = beam_scores[beam];
+    for (int i = tid; i < V; i += BT_THREADS) s_x[i] = ((s_x[i] - mx) - lse) + run;
+    __syncthreads();
+    row_top_candidates(s_x, V, Kr, (unsigned long long)j * V, tid, sm);
+
     // sort the row's Kr candidates (descending key) by rank; pad the list with 0 (below every real candidate)
     unsigned long long* out = keys_out + (size_t)beam * K;
     if (tid < Kr) {
-        const unsigned long long me = s_cand[tid];
+        const unsigned long long me = sm.cand[tid];
         int rank = 0;
-        for (int c = 0; c < Kr; ++c) rank += s_cand[c] > me;
+        for (int c = 0; c < Kr; ++c) rank += sm.cand[c] > me;
         out[rank] = me;
     } else if (tid < K) {
         out[tid] = 0ull;
     }
 }
 
+// Beam sampling (HF _beam_search with do_sample): per beam row, the warped scores w = ((x - max) - lse) / T with top-k and
+// top-p survivors (at least min_keep of each), the accumulated score acc = w + running score, and for every finite survivor
+// the Gumbel-perturbed key fp32(acc + g), g = -log(-log u) in fp64, u from Philox(seed; step, global flat index). The row's K
+// largest keys are selected as in beam_row_topk_kernel (warped-away tokens are -inf and rank by index below every finite key,
+// NaN logits below them); the candidate's score is its unperturbed acc, written beside its key.
+__global__ void __launch_bounds__(BT_THREADS, 1)
+beam_row_sample_kernel(const float* __restrict__ logits, const int32_t* __restrict__ row_of_beam, const float* __restrict__ beam_scores,
+                       int nb, int V, int K, BeamSampleParams sp, unsigned long long* __restrict__ keys_out,
+                       float* __restrict__ scores_out) {
+    extern __shared__ __align__(16) uint8_t bt_smem[];
+    float* s_x = reinterpret_cast<float*>(bt_smem);
+    __shared__ RowSmem sm;
+
+    const int tid = threadIdx.x, j = blockIdx.x, b = blockIdx.y;
+    const int beam = b * nb + j;
+    const int row = row_of_beam ? row_of_beam[beam] : beam;
+    const int Kr = K < V ? K : V;
+    const float* x = logits + (size_t)row * V;
+    const float T = sp.temperature;
+    auto key_of = [&](int i) { return order_key(s_x[i]); };
+
+    float mx, lse;
+    stage_row(x, s_x, V, tid, sm, mx, lse);
+    for (int i = tid; i < V; i += BT_THREADS) s_x[i] = __fdiv_rn((s_x[i] - mx) - lse, T);
+    __syncthreads();
+
+    // top-k: keep w >= the k-th largest w (ties kept), k = max(top_k, min_keep)
+    const int k = sp.top_k > 0 ? max(sp.top_k, sp.min_keep) : 0;
+    if (k > 0 && k < V) {
+        const uint32_t kth = radix_select<BT_THREADS, false>(V, (unsigned long long)k, tid, key_of, [](int) { return 1ull; }, sm.hist,
+                                                             &sm.prefix, &sm.above);
+        for (int i = tid; i < V; i += BT_THREADS)
+            if (order_key(s_x[i]) < kth && s_x[i] == s_x[i]) s_x[i] = -INFINITY;  // NaN stays NaN: it ranks below -inf
+        __syncthreads();
+    }
+    // top-p over fixed-point masses of e_i = exp(w_i - max w) (the rule of sample_publish_kernel); the min_keep largest w survive
+    if (sp.top_p < 1.0f) {
+        float m = -INFINITY;
+        for (int i = tid; i < V; i += BT_THREADS) m = fmaxf(m, s_x[i] == s_x[i] ? s_x[i] : -INFINITY);
+        const float wmax = block_reduce<true>(m, sm.w, tid);
+        auto e_of = [&](int i) {
+            const float w = s_x[i];
+            return (w == w && w > -INFINITY) ? expf(w - wmax) : 0.f;
+        };
+        auto mass = [&](int i) { return mass_of(e_of(i)); };
+        unsigned long long part = 0ull;
+        for (int i = tid; i < V; i += BT_THREADS) part += mass(i);
+        const unsigned long long total = block_sum<BT_THREADS, unsigned long long>(part, sm.wsum, tid);
+        unsigned long long limit = (unsigned long long)((double)total * (double)sp.top_p);
+        if (limit < 1ull) limit = 1ull;
+        const uint32_t thr = radix_select<BT_THREADS, true>(V, limit, tid, [&](int i) { return __float_as_uint(e_of(i)); }, mass, sm.hist,
+                                                            &sm.prefix, &sm.above);
+        uint32_t kmin = 0xFFFFFFFFu;
+        __syncthreads();  // every thread has read the last level's prefix before the next descent resets it
+        if (sp.min_keep > 1)
+            kmin = radix_select<BT_THREADS, false>(V, (unsigned long long)sp.min_keep, tid, key_of, [](int) { return 1ull; }, sm.hist,
+                                                   &sm.prefix, &sm.above);
+        __syncthreads();
+        for (int i = tid; i < V; i += BT_THREADS) {
+            const bool keep = __float_as_uint(e_of(i)) >= thr || order_key(s_x[i]) >= kmin;
+            if (!keep && s_x[i] == s_x[i]) s_x[i] = -INFINITY;  // e_of reads only element i: in-place is safe per thread
+        }
+        __syncthreads();
+    }
+    // perturbed keys of the finite survivors
+    const float run = beam_scores[beam];
+    const uint32_t flat_base = (uint32_t)beam * (uint32_t)V;
+    for (int i = tid; i < V; i += BT_THREADS) {
+        const float w = s_x[i];
+        if (w == w && w > -INFINITY) {
+            const float acc = w + run;
+            const unsigned long long r = philox_u64(sp.seed, sp.step, flat_base + (uint32_t)i);
+            const double u = ((double)(r >> 11) + 0.5) * 0x1.0p-53;  // (0, 1)
+            s_x[i] = (float)((double)acc - log(-log(u)));
+        }
+    }
+    __syncthreads();
+    row_top_candidates(s_x, V, Kr, (unsigned long long)j * V, tid, sm);
+
+    unsigned long long* out = keys_out + (size_t)beam * K;
+    float* out_s = scores_out + (size_t)beam * K;
+    if (tid < Kr) {
+        const unsigned long long me = sm.cand[tid];
+        int rank = 0;
+        for (int c = 0; c < Kr; ++c) rank += sm.cand[c] > me;
+        const int i = (int)(0xFFFFFFFFu - (uint32_t)(me & 0xFFFFFFFFull) - (uint32_t)(j * V));
+        const float kx = s_x[i];
+        // a finite key is a survivor: its score is acc, recomputed with the same operations; -inf and NaN carry themselves
+        out[rank] = me;
+        out_s[rank] = (kx == kx && kx > -INFINITY) ? __fdiv_rn((x[i] - mx) - lse, T) + run : kx;
+    } else if (tid < K) {
+        out[tid] = 0ull;
+        out_s[tid] = -INFINITY;
+    }
+}
+
 __global__ void __launch_bounds__(BM_THREADS)
-beam_merge_kernel(const unsigned long long* __restrict__ keys, int nb, int K, int V, float* __restrict__ out_scores,
-                  int32_t* __restrict__ out_tokens, int32_t* __restrict__ out_beams) {
+beam_merge_kernel(const unsigned long long* __restrict__ keys, const float* __restrict__ scores, int nb, int K, int V,
+                  float* __restrict__ out_scores, int32_t* __restrict__ out_tokens, int32_t* __restrict__ out_beams) {
     const int b = blockIdx.x;
     const unsigned long long* lists = keys + (size_t)b * nb * K;
     for (int c = threadIdx.x; c < nb * K; c += BM_THREADS) {
@@ -179,7 +272,8 @@ beam_merge_kernel(const unsigned long long* __restrict__ keys, int nb, int K, in
         }
         if (rank < K) {
             const uint32_t flat = 0xFFFFFFFFu - (uint32_t)(me & 0xFFFFFFFFull);
-            out_scores[(size_t)b * K + rank] = key_float((uint32_t)(me >> 32));
+            // a sampled list carries each candidate's score beside its key; a greedy key is the score itself
+            out_scores[(size_t)b * K + rank] = scores ? scores[(size_t)b * nb * K + c] : key_float((uint32_t)(me >> 32));
             out_tokens[(size_t)b * K + rank] = (int32_t)(flat % (uint32_t)V);
             out_beams[(size_t)b * K + rank] = (int32_t)(flat / (uint32_t)V);
         }
@@ -229,7 +323,39 @@ int beam_topk(const float* logits, const int32_t* row_of_beam, const float* beam
     auto* keys = reinterpret_cast<unsigned long long*>(workspace);
     beam_row_topk_kernel<<<dim3(nb, B), BT_THREADS, smem, stream>>>(logits, row_of_beam, beam_scores, nb, V, K, keys);
     B2_LAUNCH_CHECK();
-    beam_merge_kernel<<<B, BM_THREADS, 0, stream>>>(keys, nb, K, V, out_scores, out_tokens, out_beams);
+    beam_merge_kernel<<<B, BM_THREADS, 0, stream>>>(keys, nullptr, nb, K, V, out_scores, out_tokens, out_beams);
+    B2_LAUNCH_CHECK();
+    return 0;
+}
+
+size_t beam_sample_workspace_bytes(int B, int nb, int K) {
+    return (size_t)B * nb * K * (sizeof(unsigned long long) + sizeof(float));
+}
+
+int beam_sample(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
+                const BeamSampleParams& sp, void* workspace, float* out_scores, int32_t* out_tokens, int32_t* out_beams,
+                cudaStream_t stream) {
+    B2_CHECK_ARG(logits && beam_scores && workspace && out_scores && out_tokens && out_beams, "beam_sample: null argument");
+    B2_CHECK_ARG(B >= 1 && nb >= 1 && nb <= 32, "beam_sample: B=%d nb=%d (1 <= nb <= 32)", B, nb);
+    B2_CHECK_ARG(K >= 1 && K <= 128 && (long long)K <= (long long)nb * V, "beam_sample: K=%d outside [1, min(128, nb*V=%lld)]", K,
+                 (long long)nb * V);
+    const size_t smem = (size_t)V * sizeof(float);
+    B2_CHECK_ARG(V >= 1 && smem <= 200 * 1024 && (long long)B * nb * V <= 0xFFFFFFFFll,
+                 "beam_sample: vocab %d exceeds the shared-memory staging of the kernel or B*nb*V the 32-bit Philox row", V);
+    B2_CHECK_ARG(sp.temperature > 0.f, "beam_sample: temperature %g must be > 0", (double)sp.temperature);
+    B2_CHECK_ARG(sp.top_p > 0.f && sp.top_p <= 1.f, "beam_sample: top_p %g outside (0, 1]", (double)sp.top_p);
+    B2_CHECK_ARG(sp.top_k >= 0, "beam_sample: top_k %d must be >= 0", sp.top_k);
+    B2_CHECK_ARG(sp.min_keep >= 1 && sp.min_keep <= K, "beam_sample: min_keep %d outside [1, K=%d]", sp.min_keep, K);
+    static size_t attr = 0;
+    if (smem > attr) {
+        B2_CUDA_CHECK(cudaFuncSetAttribute(beam_row_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attr = smem;
+    }
+    auto* keys = reinterpret_cast<unsigned long long*>(workspace);
+    float* scores = reinterpret_cast<float*>(keys + (size_t)B * nb * K);
+    beam_row_sample_kernel<<<dim3(nb, B), BT_THREADS, smem, stream>>>(logits, row_of_beam, beam_scores, nb, V, K, sp, keys, scores);
+    B2_LAUNCH_CHECK();
+    beam_merge_kernel<<<B, BM_THREADS, 0, stream>>>(keys, scores, nb, K, V, out_scores, out_tokens, out_beams);
     B2_LAUNCH_CHECK();
     return 0;
 }

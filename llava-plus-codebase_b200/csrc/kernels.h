@@ -310,6 +310,20 @@ int row_state_set(RowState* row_dev, const RowState& v, int32_t* tok_dev, int to
 size_t beam_topk_workspace_bytes(int B, int nb, int K);
 int beam_topk(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
               void* workspace, float* out_scores, int32_t* out_tokens, int32_t* out_beams, cudaStream_t stream);
+// beam sampling: the same selection over Gumbel-perturbed keys of the warped scores (beam_row_sample_kernel in beam.cu); each
+// candidate's score is its unperturbed accumulated score. T > 0, top_k >= 0 (0 = off), top_p in (0, 1], min_keep >= 1.
+struct BeamSampleParams {
+    float temperature;
+    int top_k;
+    float top_p;
+    int min_keep;
+    unsigned long long seed;
+    uint32_t step;
+};
+size_t beam_sample_workspace_bytes(int B, int nb, int K);
+int beam_sample(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
+                const BeamSampleParams& sp, void* workspace, float* out_scores, int32_t* out_tokens, int32_t* out_beams,
+                cudaStream_t stream);
 struct KvCopyPairs {
     static constexpr int kMax = 64;
     int32_t src[kMax], dst[kMax], end[kMax];

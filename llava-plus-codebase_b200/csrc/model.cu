@@ -913,7 +913,7 @@ int b2_init(int device) {
 }
 
 const char* b2_last_error(void) { return g_err; }
-int b2_version(void) { return 7; }
+int b2_version(void) { return 8; }
 unsigned long long b2_launch_count(void) { return g_launch_count; }
 
 int b2_model_create(const b2_model_desc* desc, b2_model** out) {
@@ -1866,13 +1866,48 @@ int b2_op_beam_topk(const float* logits, const int32_t* row_of_beam, const float
     return r;
 }
 
+static BeamSampleParams beam_sample_params(const b2_beam_sampling* s, uint32_t step) {
+    BeamSampleParams p;
+    p.temperature = s->temperature;
+    p.top_k = s->top_k;
+    p.top_p = s->top_p;
+    p.min_keep = s->min_keep;
+    p.seed = s->seed;
+    p.step = step;
+    return p;
+}
+
+int b2_op_beam_sample(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
+                      const b2_beam_sampling* sampling, uint32_t step, float* out_scores, int32_t* out_tokens, int32_t* out_beams,
+                      void* stream) {
+    B2_CHECK_ARG(sampling != nullptr, "b2_op_beam_sample: null sampling");
+    B2_CHECK_ARG(B >= 1 && nb >= 1 && nb <= 32 && K >= 1 && K <= 128, "b2_op_beam_sample: B=%d nb=%d K=%d", B, nb, K);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    void* ws = nullptr;
+    B2_CUDA_CHECK(cudaMallocAsync(&ws, beam_sample_workspace_bytes(B, nb, K), st));
+    const int r = beam_sample(logits, row_of_beam, beam_scores, B, nb, V, K, beam_sample_params(sampling, step), ws, out_scores,
+                              out_tokens, out_beams, st);
+    B2_CUDA_CHECK(cudaFreeAsync(ws, st));
+    return r;
+}
+
 int b2_beam_step(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, void* stream) {
+    return b2_beam_step_ex(m, kv, a, nullptr, 0u, stream);
+}
+
+int b2_beam_step_ex(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, const b2_beam_sampling* sampling, uint32_t step, void* stream) {
     B2_CHECK_ARG(m && kv && a && kv->m == m, "b2_beam_step: bad handle");
     B2_CHECK_ARG(m->finalized, "b2_beam_step: model not finalized");
     const int B = a->B, nb = a->nb, K = a->K, n = a->B * a->nb;
     B2_CHECK_ARG(B >= 1 && nb >= 1 && nb <= 32 && n <= kv->max_batch, "b2_beam_step: B=%d x nb=%d beams exceed the cache's %d slots",
                  B, nb, kv->max_batch);
     B2_CHECK_ARG(K >= 1 && K <= 128 && (long long)K <= (long long)nb * m->d.vocab, "b2_beam_step: K=%d outside [1, min(128, nb*V)]", K);
+    // the sampling arguments are checked before the step changes the cache, as every other argument is
+    B2_CHECK_ARG(sampling == nullptr || (sampling->temperature > 0.f && sampling->top_p > 0.f && sampling->top_p <= 1.f &&
+                                         sampling->top_k >= 0 && sampling->min_keep >= 1 && sampling->min_keep <= K),
+                 "b2_beam_step_ex: bad sampling (temperature > 0, top_p in (0, 1], top_k >= 0, 1 <= min_keep <= K)");
+    B2_CHECK_ARG(sampling == nullptr || (long long)n * m->d.vocab <= 0xFFFFFFFFll,
+                 "b2_beam_step_ex: B*nb*V exceeds the 32-bit Philox row");
     B2_CHECK_ARG(a->tokens_host && a->slot_of_beam_host && a->beam_scores_host && a->out_scores_host && a->out_tokens_host &&
                  a->out_beams_host, "b2_beam_step: null array");
     std::lock_guard<std::mutex> lk(m->mu);
@@ -1894,7 +1929,7 @@ int b2_beam_step(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, void* strea
                      kv->max_seq);
     if (kv->beam_in.p == nullptr) {
         B2_TRY(kv->beam_in.alloc((size_t)2 * kv->max_batch * 4));
-        B2_TRY(kv->beam_ws.alloc(beam_topk_workspace_bytes(kv->max_batch, 1, 128)));
+        B2_TRY(kv->beam_ws.alloc(beam_sample_workspace_bytes(kv->max_batch, 1, 128)));  // >= beam_topk's
         B2_TRY(kv->beam_out.alloc((size_t)kv->max_batch * 128 * 12));
     }
     B2_TRY(ws_enter(m, st));
@@ -1912,8 +1947,12 @@ int b2_beam_step(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, void* strea
     float* o_s = kv->beam_out.as<float>();
     int32_t* o_t = reinterpret_cast<int32_t*>(o_s + B * K);
     int32_t* o_b = o_t + B * K;
-    B2_TRY(beam_topk(m->logits.as<float>(), rows, reinterpret_cast<const float*>(rows + kv->max_batch), B, nb, m->d.vocab, K, kv->beam_ws.p,
-                     o_s, o_t, o_b, st));
+    const float* run_scores = reinterpret_cast<const float*>(rows + kv->max_batch);
+    if (sampling != nullptr)
+        B2_TRY(beam_sample(m->logits.as<float>(), rows, run_scores, B, nb, m->d.vocab, K, beam_sample_params(sampling, step), kv->beam_ws.p,
+                           o_s, o_t, o_b, st));
+    else
+        B2_TRY(beam_topk(m->logits.as<float>(), rows, run_scores, B, nb, m->d.vocab, K, kv->beam_ws.p, o_s, o_t, o_b, st));
     B2_CUDA_CHECK(cudaMemcpyAsync(a->out_scores_host, o_s, (size_t)B * K * 4, cudaMemcpyDeviceToHost, st));
     B2_CUDA_CHECK(cudaMemcpyAsync(a->out_tokens_host, o_t, (size_t)B * K * 4, cudaMemcpyDeviceToHost, st));
     B2_CUDA_CHECK(cudaMemcpyAsync(a->out_beams_host, o_b, (size_t)B * K * 4, cudaMemcpyDeviceToHost, st));

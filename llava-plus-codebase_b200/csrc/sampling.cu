@@ -20,48 +20,16 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "select.cuh"
 
 namespace b2 {
 namespace {
 
 constexpr int SP_THREADS = 1024;
-constexpr float SP_FIXED_ONE = 1099511627776.0f;  // 2^40: probability mass in fixed point
 
 __device__ __forceinline__ uint32_t order_key(float x) {  // monotone float -> uint (x < y  <=>  key(x) < key(y))
     const uint32_t u = __float_as_uint(x);
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ unsigned long long mass_of(float e) {
-    return e > 0.f ? __float2ull_rz(e * SP_FIXED_ONE) : 0ull;  // NaN / -inf survivors carry no mass
-}
-
-__device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c[0]), lo0 = 0xD2511F53u * c[0];
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c[2]), lo1 = 0xCD9E8D57u * c[2];
-    const uint32_t n0 = hi1 ^ c[1] ^ k0, n1 = lo1, n2 = hi0 ^ c[3] ^ k1, n3 = lo0;
-    c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
-}
-__device__ __forceinline__ unsigned long long philox_u64(unsigned long long seed, uint32_t index, uint32_t row) {
-    uint32_t c[4] = {index, row, 0u, 0u};
-    uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        philox_round(c, k0, k1);
-        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-    }
-    return ((unsigned long long)c[0] << 32) | c[1];
-}
-
-template <typename T>
-__device__ __forceinline__ T block_sum(T v, T* s_w, int tid) {  // fixed order: warp shuffle tree, then warp sums in order
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    __syncthreads();
-    if ((tid & 31) == 0) s_w[tid >> 5] = v;
-    __syncthreads();
-    T t = 0;
-    for (int i = 0; i < SP_THREADS / 32; ++i) t += s_w[i];
-    return t;
 }
 
 // argmax with torch.argmax tie-breaking (value desc, index asc), NaN skipped; result valid in every thread
@@ -89,54 +57,6 @@ __device__ __forceinline__ int block_argmax(const float* row, int V, int tid, fl
     }
     if (max_out) *max_out = best;
     return bi == INT_MAX ? 0 : bi;
-}
-
-// Radix descent, 8 bits per level from the top. Level state lives in shared memory (s_prefix / s_above).
-//   COUNT mode (top-k): weight of an element = 1; selects the key of the k-th largest element.
-//   MASS  mode (top-p): weight = mass_of(e); selects the smallest key whose strictly-above mass is < limit.
-template <bool MASS>
-__device__ __forceinline__ uint32_t radix_select(const float* s_x, int V, unsigned long long limit, int tid,
-                                                 unsigned long long* s_hist, uint32_t* s_prefix,
-                                                 unsigned long long* s_above) {
-    if (tid == 0) { *s_prefix = 0u; *s_above = 0ull; }
-    for (int level = 0; level < 4; ++level) {
-        const int shift = 24 - 8 * level;
-        if (tid < 256) s_hist[tid] = 0ull;
-        __syncthreads();
-        const uint32_t prefix = *s_prefix;
-        for (int i = tid; i < V; i += SP_THREADS) {
-            const float x = s_x[i];
-            const uint32_t key = MASS ? __float_as_uint(x > 0.f ? x : 0.f) : order_key(x);
-            if (level == 0 || (key >> (shift + 8)) == prefix) {
-                const unsigned long long w = MASS ? mass_of(x) : 1ull;
-                if (w) atomicAdd(&s_hist[(key >> shift) & 255u], w);  // integer adds: order-independent
-            }
-        }
-        __syncthreads();
-        if (tid == 0) {
-            unsigned long long acc = *s_above;
-            int pick = 255;
-            if (MASS) {
-                // smallest digit d whose strictly-above mass acc_d is still < limit (acc_255 = above < limit by construction)
-                for (int d = 255; d >= 0; --d) {
-                    if (acc >= limit) break;
-                    pick = d;
-                    *s_above = acc;
-                    acc += s_hist[d];
-                }
-            } else {
-                // digit holding the limit-th largest element: walk down until the running count reaches it
-                pick = 0;
-                for (int d = 255; d >= 0; --d) {
-                    if (acc + s_hist[d] >= limit) { pick = d; *s_above = acc; break; }
-                    acc += s_hist[d];
-                }
-            }
-            *s_prefix = (prefix << 8) | (uint32_t)pick;
-        }
-        __syncthreads();
-    }
-    return *s_prefix;
 }
 
 // HF's history-aware processors over the staged row s_x, in transformers' order (repetition -> no-repeat-ngram -> min_length /
@@ -272,7 +192,9 @@ sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleStat
         // ---- top-k: keep everything >= the k-th largest scaled logit (ties kept, like TopKLogitsWarper) ----
         const int k = top_k;
         if (k > 0 && k < V) {
-            const uint32_t kth = radix_select<false>(s_x, V, (unsigned long long)k, tid, s_hist, &s_prefix, &s_above);
+            const uint32_t kth = radix_select<SP_THREADS, false>(
+                V, (unsigned long long)k, tid, [&](int i) { return order_key(s_x[i]); }, [](int) { return 1ull; }, s_hist,
+                &s_prefix, &s_above);
             for (int i = tid; i < V; i += SP_THREADS)
                 if (order_key(s_x[i]) < kth) s_x[i] = -INFINITY;
             __syncthreads();
@@ -289,10 +211,12 @@ sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleStat
         if (top_p < 1.0f) {
             unsigned long long part = 0ull;
             for (int i = tid; i < V; i += SP_THREADS) part += mass_of(s_x[i]);
-            const unsigned long long total = block_sum<unsigned long long>(part, s_wsum, tid);
+            const unsigned long long total = block_sum<SP_THREADS, unsigned long long>(part, s_wsum, tid);
             unsigned long long limit = (unsigned long long)((double)total * (double)(top_p > 0.f ? top_p : 0.f));
             if (limit < 1ull) limit = 1ull;  // min_tokens_to_keep = 1: the largest probability always survives
-            const uint32_t thr = radix_select<true>(s_x, V, limit, tid, s_hist, &s_prefix, &s_above);
+            const uint32_t thr = radix_select<SP_THREADS, true>(
+                V, limit, tid, [&](int i) { const float x = s_x[i]; return __float_as_uint(x > 0.f ? x : 0.f); },
+                [&](int i) { return mass_of(s_x[i]); }, s_hist, &s_prefix, &s_above);
             for (int i = tid; i < V; i += SP_THREADS) {
                 const float x = s_x[i];
                 if (__float_as_uint(x > 0.f ? x : 0.f) < thr) s_x[i] = 0.f;

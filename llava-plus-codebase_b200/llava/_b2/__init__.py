@@ -62,6 +62,17 @@ class BeamStepArgs(_c.Structure):
                 ("beam_scores_host", _vp), ("out_scores_host", _vp), ("out_tokens_host", _vp), ("out_beams_host", _vp)]
 
 
+class BeamSampling(_c.Structure):
+    """b2_beam_sampling (include/b2llava.h): warpers and Philox key of beam sampling."""
+    _fields_ = [("temperature", _c.c_float), ("top_k", _c.c_int32), ("top_p", _c.c_float), ("min_keep", _c.c_int32),
+                ("seed", _c.c_ulonglong)]
+
+
+def make_beam_sampling(temperature=1.0, top_k=50, top_p=1.0, min_keep=2, seed=0):
+    return BeamSampling(float(temperature), int(top_k or 0), float(1.0 if top_p is None else top_p), int(min_keep),
+                        int(seed) & (2**64 - 1))
+
+
 class LogitsProc(_c.Structure):
     """b2_logits_proc (include/b2llava.h): history-aware logits processors of one row; `prompt_ids` is a device int64 pointer."""
     _fields_ = [("repetition_penalty", _c.c_float), ("no_repeat_ngram_size", _c.c_int32), ("min_generated", _c.c_int32),
@@ -181,6 +192,8 @@ SIGNATURES = {
     "b2_kv_copy_slots": (_i32, [_vp, _vp, _c.POINTER(_c.c_int32), _c.POINTER(_c.c_int32), _i32, _i32, _vp]),
     "b2_op_beam_topk": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     "b2_beam_step": (_i32, [_vp, _vp, _c.POINTER(BeamStepArgs), _vp]),
+    "b2_op_beam_sample": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _c.POINTER(BeamSampling), _c.c_uint32, _vp, _vp, _vp, _vp]),
+    "b2_beam_step_ex": (_i32, [_vp, _vp, _c.POINTER(BeamStepArgs), _c.POINTER(BeamSampling), _c.c_uint32, _vp]),
     "b2_op_gemm": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "b2_op_gemv": (_i32, [_vp, _i64, _vp, _i32, _vp, _f32, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "b2_op_quantize_nf4": (_i32, [_vp, _i32, _i32, _vp, _vp, _vp]),
@@ -606,10 +619,26 @@ class Engine:
                                            ptr(out_b), stream_ptr()), "b2_op_beam_topk")
         return out_s, out_t, out_b
 
-    def beam_step(self, kv, copies, row_begin, tokens, slot_of_beam, beam_scores, nb, K):
-        """One step of the running beams (b2_beam_step): `copies` = [(src, dst)] applied first, tokens[i] fed to slot
-        slot_of_beam[i], one decode step at batch len(tokens), candidates of every sample selected on the device. Returns CPU
-        tensors (scores fp32, tokens int64, beams int64), each [B, K], best first."""
+    def beam_sample(self, logits, beam_scores, nb, K, sampling, step, row_of_beam=None):
+        """beam_topk with the candidates drawn without replacement (b2_op_beam_sample): `sampling` a BeamSampling, `step` the
+        index of the draw. Returns device tensors (scores fp32, tokens int32, beams int32), each [B, K], in draw order."""
+        V = logits.shape[-1]
+        scores = beam_scores.to(device=self.device, dtype=torch.float32).contiguous()
+        B = scores.numel() // nb
+        rows = None if row_of_beam is None else torch.as_tensor(row_of_beam, dtype=torch.int32).to(self.device).contiguous()
+        out_s = torch.empty(B, K, dtype=torch.float32, device=self.device)
+        out_t = torch.empty(B, K, dtype=torch.int32, device=self.device)
+        out_b = torch.empty(B, K, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.index):
+            check(self.lib.b2_op_beam_sample(ptr(logits), ptr(rows), ptr(scores), B, int(nb), V, int(K), ctypes.byref(sampling),
+                                             int(step), ptr(out_s), ptr(out_t), ptr(out_b), stream_ptr()), "b2_op_beam_sample")
+        return out_s, out_t, out_b
+
+    def beam_step(self, kv, copies, row_begin, tokens, slot_of_beam, beam_scores, nb, K, sampling=None, step=0):
+        """One step of the running beams (b2_beam_step, or b2_beam_step_ex with a BeamSampling): `copies` = [(src, dst)] applied
+        first, tokens[i] fed to slot slot_of_beam[i], one decode step at batch len(tokens), candidates of every sample selected
+        (or, with `sampling`, drawn as draw `step`) on the device. Returns CPU tensors (scores fp32, tokens int64, beams int64),
+        each [B, K], best (or first drawn) first."""
         n = len(tokens)
         B = n // nb
         i32 = lambda xs: (_c.c_int32 * max(len(xs), 1))(*[int(x) for x in xs])
@@ -623,7 +652,11 @@ class Engine:
                          _c.cast(slots, _vp), _c.cast(scores, _vp), _vp(out_s.data_ptr()), _vp(out_t.data_ptr()),
                          _vp(out_b.data_ptr()))
         with torch.cuda.device(self.index):
-            check(self.lib.b2_beam_step(self.handle, kv.handle, ctypes.byref(a), stream_ptr()), "b2_beam_step")
+            if sampling is None:
+                check(self.lib.b2_beam_step(self.handle, kv.handle, ctypes.byref(a), stream_ptr()), "b2_beam_step")
+            else:
+                check(self.lib.b2_beam_step_ex(self.handle, kv.handle, ctypes.byref(a), ctypes.byref(sampling), int(step),
+                                               stream_ptr()), "b2_beam_step_ex")
         return out_s, out_t.long(), out_b.long()
 
     def argmax(self, logits):

@@ -27,7 +27,7 @@ from ..llava_arch import LlavaMetaModel, LlavaMetaForCausalLM
 from ..multimodal_encoder.clip_encoder import _Holder, _read_checkpoint_dir
 from ..._b2 import (Engine, KVCache, LOGITS_ALL, LOGITS_LAST, ERR_SPLICE_SLOTS, INT32_MIN, kv_dtype_code, last_error, make_logits_proc,
                      make_prompt_lookup,
-                    make_sampling)
+                    make_sampling, make_beam_sampling)
 from ..._b2 import prefix as _prefix
 from ...constants import IMAGE_TOKEN_INDEX
 from ..llava_arch import build_source_index
@@ -512,8 +512,8 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                                           "min_length) together with num_beams > 1 are not implemented on the H100 path")
             if self._beam_search_cap() < 2:
                 raise NotImplementedError("beam search is not used on the LLaVA path (num_beams=1 everywhere)")
-            beam_args = self._beam_arguments(num_beams, do_sample, temperature, streamer, output_scores, return_dict_in_generate,
-                                             kwargs)
+            beam_args = self._beam_arguments(num_beams, do_sample, temperature, top_p, top_k, streamer, output_scores,
+                                             return_dict_in_generate, kwargs)
         if return_dict_in_generate or output_scores:
             raise NotImplementedError("generate() returns the id tensor only")
         prompt = inputs if inputs.dim() == 2 else inputs.unsqueeze(0)
@@ -773,12 +773,23 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         except (TypeError, ValueError):
             raise ValueError(f"b2_beam_search must be an integer, got {v!r}")
 
-    def _beam_arguments(self, num_beams, do_sample, temperature, streamer, output_scores, return_dict_in_generate, kwargs):
-        """Checks what generate(num_beams > 1) does not implement and takes the beam-only arguments out of `kwargs`."""
+    def _beam_sample_on(self):
+        """config.b2_beam_sample or B2_BEAM_SAMPLE=1: generate(do_sample=True, num_beams > 1) runs beam sampling (off by default:
+        its draws come from the engine's Philox stream, so a seeded run equals transformers' in distribution, not in ids)."""
+        v = getattr(self.config, "b2_beam_sample", None)
+        return bool(v) if v is not None else os.environ.get("B2_BEAM_SAMPLE") == "1"
+
+    def _beam_arguments(self, num_beams, do_sample, temperature, top_p, top_k, streamer, output_scores, return_dict_in_generate,
+                        kwargs):
+        """Checks what generate(num_beams > 1) does not implement and takes the beam-only arguments out of `kwargs`. With
+        do_sample (and a temperature above 1e-5, below which it is beam search) the result carries `sampling`: the warpers of
+        beam sampling, HF GenerationConfig's defaults top_k = 50 and top_p = 1.0 filled in."""
         if num_beams < 1 or num_beams > self._beam_search_cap():
             raise ValueError(f"num_beams={num_beams} exceeds config.b2_beam_search={self._beam_search_cap()}")
-        if do_sample and not (temperature is not None and temperature <= 1e-5):
-            raise NotImplementedError("beam sampling (do_sample=True with num_beams > 1) is not implemented on the H100 path")
+        sampled = bool(do_sample) and not (temperature is not None and temperature <= 1e-5)
+        if sampled and not self._beam_sample_on():
+            raise NotImplementedError("beam sampling (do_sample=True with num_beams > 1) is not implemented on the H100 path "
+                                      "without config.b2_beam_sample")
         if (kwargs.get("num_beam_groups") or 1) != 1 or (kwargs.get("diversity_penalty") or 0.0) != 0.0:
             raise NotImplementedError("group beam search (num_beam_groups / diversity_penalty) is not implemented on the H100 path")
         if kwargs.get("constraints") is not None:
@@ -787,17 +798,30 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             raise NotImplementedError("beam search returns the id tensor only (output_scores / return_dict_in_generate)")
         if streamer is not None:
             raise ValueError("`streamer` cannot be used with beam search (num_beams > 1)")
+        sampling = None
+        if sampled:
+            if top_p is not None and not (0.0 < top_p <= 1.0):
+                raise ValueError(f"top_p must be in (0, 1], got {top_p}")
+            if top_k is not None and int(top_k) < 0:
+                raise ValueError(f"top_k must be a non-negative integer, got {top_k}")
+            sampling = dict(temperature=1.0 if temperature is None else float(temperature), top_k=50 if top_k is None else int(top_k),
+                            top_p=1.0 if top_p is None else float(top_p))
         lp = kwargs.pop("length_penalty", None)
         es = kwargs.pop("early_stopping", None)
         nrs = kwargs.pop("num_return_sequences", None)
         return dict(length_penalty=1.0 if lp is None else float(lp), early_stopping=False if es is None else es,
-                    num_return_sequences=1 if nrs is None else int(nrs))
+                    num_return_sequences=1 if nrs is None else int(nrs), sampling=sampling)
 
     def _beam_generate(self, engine, prompt, images, attention_mask, num_beams, max_new_tokens, eos_ids, pad_token_id,
-                       stopping_criteria, length_penalty, early_stopping, num_return_sequences):
+                       stopping_criteria, length_penalty, early_stopping, num_return_sequences, sampling=None):
         """Beam search (llava/_b2/beam.py): sample b is prefilled once into slot b of a pool cache; its candidates from the
         prefill logits fork the prompt into nb slots; then every b2_beam_step applies the step's slot copies, decodes the
-        B * nb running beams in one batch and returns the K best candidates per sample for the host bookkeeping."""
+        B * nb running beams in one batch and returns the K best candidates per sample for the host bookkeeping.
+
+        With `sampling` (beam sampling) the device draws the K candidates of step t with b2_op_beam_sample / b2_beam_step_ex at
+        draw index t, seeded from torch's CPU generator. The first draw reads all nb beam rows of a sample, each mapped to its
+        prefill row, with running scores [0, -1e9, ...] as HF's first step does: the -1e9 rows matter to which candidates fill
+        the list when fewer than K have positive probability."""
         from ..._b2 import beam as _beam
 
         B = prompt.shape[0]
@@ -806,6 +830,12 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                                   pad_token_id, stopping_criteria)
         if engine.vocab < search.K:
             raise ValueError(f"beam search keeps {search.K} candidates per step, more than the vocabulary ({engine.vocab})")
+        bs = None
+        if sampling is not None:
+            # HF _get_logits_processor: min_tokens_to_keep = 1 + number of eos ids, 2 when there are none
+            min_keep = 2 if eos_ids is None else 1 + len(eos_ids)
+            seed = int(torch.randint(0, 2**62, (1,), dtype=torch.int64).item())
+            bs = make_beam_sampling(sampling["temperature"], sampling["top_k"], sampling["top_p"], min_keep, seed)
         self._check_limits(engine, B * nb, 1)
         kv = self._pool.acquire()  # exclusive for this call; never recorded for prefix reuse
         try:
@@ -814,7 +844,12 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 self._check_limits(engine, B * nb, max(lens) + max_new_tokens)
                 kv.reset()
                 logits = engine.prefill(kv, embeds, lens, LOGITS_LAST)
-                cand = [t.cpu() for t in engine.beam_topk(logits, torch.zeros(B), 1, search.K)]  # synchronises
+                if bs is None:
+                    cand = [t.cpu() for t in engine.beam_topk(logits, torch.zeros(B), 1, search.K)]  # synchronises
+                else:
+                    cand = [t.cpu() for t in engine.beam_sample(logits, search.running_scores.reshape(-1), nb, search.K, bs, 0,
+                                                                row_of_beam=[b for b in range(B) for _ in range(nb)])]
+                    cand[2].zero_()  # every beam still holds the bare prompt, which only slot b has: all descend from beam 0
                 return cand, lens, speculative
 
             cand, lens, speculative = first_candidates(False)
@@ -826,10 +861,12 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 raise ValueError(last_error())
             planner = _beam.SlotPlanner(B, nb)
             row_begin = 0  # the first plan copies whole prompts; later ones only rows behind the shortest prompt
+            step = 0
             while not search.step(*cand):
+                step += 1
                 copies = planner.plan(search.parents)
                 cand = engine.beam_step(kv, copies, row_begin, search.next_tokens().tolist(), planner.flat(),
-                                        search.running_scores.reshape(-1).tolist(), nb, search.K)
+                                        search.running_scores.reshape(-1).tolist(), nb, search.K, sampling=bs, step=step)
                 row_begin = min(lens)
             engine.check_async_error()
         finally:
