@@ -1,9 +1,4 @@
-// Attention kernels.
-//   flash_attn_bf16  : prefill / ViT attention, flash-style online softmax, never materialises the
-//                      [B,H,S,S] score matrix the reference's eager path builds
-//                      (transformers modeling_llama.py:199-221 eager_attention_forward, modeling_clip.py:261-279).
-//                      bf16 operands, fp32 softmax statistics and accumulators. Round-1 implementation uses
-//                      mma.sync m16n8k16 (HMMA) tiles; it is <2% of prefill FLOPs (SURVEY §8a).
+// Attention kernels besides the prefill / ViT flash attention (attention_wgmma.cu).
 //   rope_kv_write    : RoPE (modeling_llama.py:124-168, half-split rotate_half) on q,k of a prefill chunk and
 //                      the KV-cache write (modeling_llama.py:269-270 cache update).
 //   decode_attn_bf16 : one-token decode: RoPE + cache append + split-KV attention with coalesced 16-byte
@@ -13,8 +8,6 @@
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>
 #include <math.h>
-
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -51,197 +44,6 @@ __device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a
         "{%0,%1,%2,%3};"
         : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-// ------------------------------------------------------------------------------------------------
-// flash attention forward (prefill / ViT)
-// ------------------------------------------------------------------------------------------------
-constexpr int FA_BM = 64;  // query rows per CTA (4 warps x 16)
-constexpr int FA_BN = 64;  // keys per tile
-
-struct FlashParams {
-    const __nv_bfloat16* q; int64_t q_bs, q_ts, q_hs;
-    const __nv_bfloat16* k; int64_t k_bs, k_ts, k_hs;
-    const __nv_bfloat16* v; int64_t v_bs, v_ts, v_hs;
-    __nv_bfloat16* o;       int64_t o_bs, o_ts, o_hs;
-    const int32_t* seq_lens;
-    int S;
-    float scale_log2;
-};
-
-template <int D, bool CAUSAL>
-__global__ void __launch_bounds__(128) flash_fwd_kernel(FlashParams p) {
-    constexpr int LD = D + 8;  // padded smem row (elements): 16B-aligned rows, conflict-free ldmatrix
-    extern __shared__ __align__(16) uint8_t fa_smem[];
-    __nv_bfloat16* sQ = reinterpret_cast<__nv_bfloat16*>(fa_smem);  // [64][LD]
-    __nv_bfloat16* sK = sQ + FA_BM * LD;                            // [2][64][LD]
-    __nv_bfloat16* sV = sK + 2 * FA_BN * LD;                        // [2][64][LD]
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int q0 = blockIdx.x * FA_BM;
-    const int head = blockIdx.y, b = blockIdx.z;
-    const int len = p.seq_lens != nullptr ? p.seq_lens[b] : p.S;  // valid keys of this sample
-    const int kv_end = CAUSAL ? min(len, q0 + FA_BM) : len;
-    const int n_tiles = (kv_end + FA_BN - 1) / FA_BN;
-
-    const __nv_bfloat16* qg = p.q + b * p.q_bs + head * p.q_hs;
-    const __nv_bfloat16* kg = p.k + b * p.k_bs + head * p.k_hs;
-    const __nv_bfloat16* vg = p.v + b * p.v_bs + head * p.v_hs;
-
-    constexpr int CHUNKS = D / 8;  // 16B chunks per row
-    auto load_q = [&]() {
-        for (int i = tid; i < FA_BM * CHUNKS; i += 128) {
-            const int r = i / CHUNKS, c = i % CHUNKS;
-            const int t = q0 + r;
-            cp_async_16(sQ + r * LD + c * 8, qg + (int64_t)min(t, p.S - 1) * p.q_ts + c * 8, t < p.S);
-        }
-    };
-    auto load_kv = [&](int tile, int buf) {
-        __nv_bfloat16* dk = sK + buf * FA_BN * LD;
-        __nv_bfloat16* dv = sV + buf * FA_BN * LD;
-        for (int i = tid; i < FA_BN * CHUNKS; i += 128) {
-            const int r = i / CHUNKS, c = i % CHUNKS;
-            const int t = tile * FA_BN + r;
-            const bool ok = t < len;
-            const int tt = ok ? t : 0;
-            cp_async_16(dk + r * LD + c * 8, kg + (int64_t)tt * p.k_ts + c * 8, ok);
-            cp_async_16(dv + r * LD + c * 8, vg + (int64_t)tt * p.v_ts + c * 8, ok);
-        }
-    };
-
-    load_q();
-    if (n_tiles > 0) load_kv(0, 0);
-    cp_async_commit();
-
-    uint32_t qf[D / 16][4];
-    float oacc[D / 8][4];
-#pragma unroll
-    for (int i = 0; i < D / 8; ++i) oacc[i][0] = oacc[i][1] = oacc[i][2] = oacc[i][3] = 0.f;
-    float m_run[2] = {-INFINITY, -INFINITY};
-    float l_run[2] = {0.f, 0.f};
-
-    const int g = lane >> 2, tq = lane & 3;
-    const int qrow0 = q0 + warp * 16 + g;  // this thread's rows: qrow0 and qrow0 + 8
-
-    for (int j = 0; j < n_tiles; ++j) {
-        if (j + 1 < n_tiles) load_kv(j + 1, (j + 1) & 1);
-        cp_async_commit();
-        cp_async_wait<1>();
-        __syncthreads();
-        if (j == 0) {
-#pragma unroll
-            for (int kk = 0; kk < D / 16; ++kk) {
-                const int r = warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
-                const int c = kk * 16 + (lane >> 4) * 8;
-                ldmatrix_x4(qf[kk], sQ + r * LD + c);
-            }
-        }
-        const __nv_bfloat16* tK = sK + (j & 1) * FA_BN * LD;
-        const __nv_bfloat16* tV = sV + (j & 1) * FA_BN * LD;
-
-        // ---- S = Q K^T (16 x 64 per warp) ----
-        float s[FA_BN / 8][4];
-#pragma unroll
-        for (int nt = 0; nt < FA_BN / 8; ++nt) s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk) {
-#pragma unroll
-            for (int np = 0; np < FA_BN / 16; ++np) {
-                uint32_t bfr[4];
-                const int r = np * 16 + (lane & 7) + (lane >> 4) * 8;  // key row
-                const int c = kk * 16 + ((lane >> 3) & 1) * 8;         // d column
-                ldmatrix_x4(bfr, tK + r * LD + c);
-                mma_bf16_16816(s[2 * np], qf[kk], bfr[0], bfr[1]);
-                mma_bf16_16816(s[2 * np + 1], qf[kk], bfr[2], bfr[3]);
-            }
-        }
-
-        // ---- scale, mask, online softmax ----
-        const int key0 = j * FA_BN;
-        float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-        for (int nt = 0; nt < FA_BN / 8; ++nt) {
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const int key = key0 + nt * 8 + tq * 2 + (e & 1);
-                const int qr = qrow0 + (e >> 1) * 8;
-                bool ok = key < len;
-                if (CAUSAL) ok = ok && (key <= qr);
-                const float val = ok ? s[nt][e] * p.scale_log2 : -INFINITY;
-                s[nt][e] = val;
-                mx[e >> 1] = fmaxf(mx[e >> 1], val);
-            }
-        }
-        float corr[2], m_use[2];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
-            mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
-            const float m_new = fmaxf(m_run[h], mx[h]);
-            m_use[h] = (m_new == -INFINITY) ? 0.f : m_new;
-            corr[h] = exp2f(m_run[h] - m_use[h]);  // m_run = -inf -> 0
-            m_run[h] = m_new;
-            l_run[h] *= corr[h];
-        }
-        float rs[2] = {0.f, 0.f};
-#pragma unroll
-        for (int nt = 0; nt < FA_BN / 8; ++nt) {
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float pv = exp2f(s[nt][e] - m_use[e >> 1]);
-                s[nt][e] = pv;
-                rs[e >> 1] += pv;
-            }
-        }
-        l_run[0] += rs[0];
-        l_run[1] += rs[1];
-#pragma unroll
-        for (int i = 0; i < D / 8; ++i) {
-            oacc[i][0] *= corr[0]; oacc[i][1] *= corr[0];
-            oacc[i][2] *= corr[1]; oacc[i][3] *= corr[1];
-        }
-
-        // ---- O += P V ----
-#pragma unroll
-        for (int kk = 0; kk < FA_BN / 16; ++kk) {
-            uint32_t pa[4];
-            pa[0] = pack_bf16(s[2 * kk][0], s[2 * kk][1]);
-            pa[1] = pack_bf16(s[2 * kk][2], s[2 * kk][3]);
-            pa[2] = pack_bf16(s[2 * kk + 1][0], s[2 * kk + 1][1]);
-            pa[3] = pack_bf16(s[2 * kk + 1][2], s[2 * kk + 1][3]);
-#pragma unroll
-            for (int dp = 0; dp < D / 16; ++dp) {
-                uint32_t bfr[4];
-                const int r = kk * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;  // key row
-                const int c = dp * 16 + (lane >> 4) * 8;                      // d column
-                ldmatrix_x4_trans(bfr, tV + r * LD + c);
-                mma_bf16_16816(oacc[2 * dp], pa, bfr[0], bfr[1]);
-                mma_bf16_16816(oacc[2 * dp + 1], pa, bfr[2], bfr[3]);
-            }
-        }
-        __syncthreads();  // everyone done with buffer (j&1) before it is refilled at iteration j+1
-    }
-    cp_async_wait<0>();
-
-    // ---- finalise ----
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
-        l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
-    }
-    __nv_bfloat16* og = p.o + b * p.o_bs + head * p.o_hs;
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-        const int t = qrow0 + h * 8;
-        if (t < p.S) {
-            const float inv = l_run[h] > 0.f ? 1.f / l_run[h] : 0.f;
-#pragma unroll
-            for (int i = 0; i < D / 8; ++i) {
-                const uint32_t pk = pack_bf16(oacc[i][2 * h] * inv, oacc[i][2 * h + 1] * inv);
-                *reinterpret_cast<uint32_t*>(og + (int64_t)t * p.o_ts + i * 8 + tq * 2) = pk;
-            }
-        }
-    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1057,47 +859,6 @@ __global__ void __launch_bounds__(DA_THREADS) decode_attn_e4m3_kernel(DecodeAttn
 }
 
 }  // namespace
-
-int flash_attn_bf16(const FlashArgs& a, cudaStream_t stream) {
-    B2_CHECK_ARG(a.D == 64 || a.D == 128, "flash_attn: head_dim must be 64 or 128 (got %d)", a.D);
-    B2_CHECK_ARG(a.B > 0 && a.H > 0 && a.S > 0, "flash_attn: empty problem");
-    // wgmma kernel unless B2_FLASH_TC=0 selects the mma.sync one (A/B knob, re-read per call: scripts/attn_bench.py)
-    const char* e = getenv("B2_FLASH_TC");
-    const bool use_tc = e == nullptr || e[0] != '0';
-    B2_CHECK_ARG(use_tc || a.pos0 == nullptr, "flash_attn: queries at a cache offset need the wgmma kernel (B2_FLASH_TC=0 is set)");
-    return use_tc ? flash_attn_tc_bf16(a, stream) : flash_attn_mma_bf16(a, stream);
-}
-
-int flash_attn_mma_bf16(const FlashArgs& a, cudaStream_t stream) {
-    FlashParams p;
-    p.q = reinterpret_cast<const __nv_bfloat16*>(a.q); p.q_bs = a.q_bs; p.q_ts = a.q_ts; p.q_hs = a.q_hs;
-    p.k = reinterpret_cast<const __nv_bfloat16*>(a.k); p.k_bs = a.k_bs; p.k_ts = a.k_ts; p.k_hs = a.k_hs;
-    p.v = reinterpret_cast<const __nv_bfloat16*>(a.v); p.v_bs = a.v_bs; p.v_ts = a.v_ts; p.v_hs = a.v_hs;
-    p.o = reinterpret_cast<__nv_bfloat16*>(a.o);       p.o_bs = a.o_bs; p.o_ts = a.o_ts; p.o_hs = a.o_hs;
-    p.seq_lens = a.seq_lens;
-    p.S = a.S;
-    p.scale_log2 = a.scale * 1.4426950408889634f;
-    dim3 grid((a.S + FA_BM - 1) / FA_BM, a.H, a.B);
-    const int smem = (FA_BM + 4 * FA_BN) * (a.D + 8) * 2;
-#define B2_FA_LAUNCH(DD, CC)                                                                              \
-    do {                                                                                                  \
-        static bool attr_set = false;                                                                     \
-        if (!attr_set) {                                                                                  \
-            B2_CUDA_CHECK(cudaFuncSetAttribute(flash_fwd_kernel<DD, CC>,                                  \
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize, smem));       \
-            attr_set = true;                                                                              \
-        }                                                                                                 \
-        flash_fwd_kernel<DD, CC><<<grid, 128, smem, stream>>>(p);                                         \
-    } while (0)
-    if (a.D == 64) {
-        if (a.causal) B2_FA_LAUNCH(64, true); else B2_FA_LAUNCH(64, false);
-    } else {
-        if (a.causal) B2_FA_LAUNCH(128, true); else B2_FA_LAUNCH(128, false);
-    }
-#undef B2_FA_LAUNCH
-    B2_LAUNCH_CHECK();
-    return 0;
-}
 
 int rope_table_build(void* table, int Smax, int D, float theta, cudaStream_t stream) {
     B2_CHECK_ARG(table != nullptr && Smax > 0 && D > 0 && D % 2 == 0, "rope_table_build: bad argument");

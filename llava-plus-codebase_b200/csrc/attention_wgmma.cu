@@ -242,7 +242,7 @@ int make_tmap_4d(CUtensorMap* map, const void* ptr, int D, int S, int H, int B, 
         fn = reinterpret_cast<PFN_encodeTiled>(f);
     }
     if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0 || (ts * 2) % 16 != 0 || (hs * 2) % 16 != 0 || (bs * 2) % 16 != 0) {
-        set_error("flash_attn(tc): operands must be 16B aligned with 16B-multiple strides");
+        set_error("flash_attn: operands must be 16B aligned with 16B-multiple strides");
         return -1;
     }
     cuuint64_t dims[4] = {(cuuint64_t)D, (cuuint64_t)S, (cuuint64_t)H, (cuuint64_t)B};
@@ -289,13 +289,14 @@ int launch_tc(const FlashArgs& a, cudaStream_t stream) {
 
 }  // namespace
 
-int flash_attn_tc_bf16(const FlashArgs& a, cudaStream_t stream) {
-    B2_CHECK_ARG(a.D == 64 || a.D == 128, "flash_attn(tc): head_dim must be 64 or 128 (got %d)", a.D);
+int flash_attn_bf16(const FlashArgs& a, cudaStream_t stream) {
+    B2_CHECK_ARG(a.D == 64 || a.D == 128, "flash_attn: head_dim must be 64 or 128 (got %d)", a.D);
+    B2_CHECK_ARG(a.B > 0 && a.H > 0 && a.S > 0, "flash_attn: empty problem");
     B2_CHECK_ARG((a.o_ts % 8) == 0 && (a.o_hs % 8) == 0 && (a.o_bs % 8) == 0 && (reinterpret_cast<uintptr_t>(a.o) & 15) == 0,
-                 "flash_attn(tc): output must be 16B aligned with 16B-multiple strides");
+                 "flash_attn: output must be 16B aligned with 16B-multiple strides");
     if (a.pos0 != nullptr) {
         // chunk against a cache: causal, head_dim 128 (the decoder's attention) only
-        B2_CHECK_ARG(a.D == 128 && a.causal && a.Skv >= 1, "flash_attn(tc): offset queries need D=128, causal, Skv >= 1 (D=%d causal=%d Skv=%d)",
+        B2_CHECK_ARG(a.D == 128 && a.causal && a.Skv >= 1, "flash_attn: offset queries need D=128, causal, Skv >= 1 (D=%d causal=%d Skv=%d)",
                      a.D, a.causal, a.Skv);
         return launch_tc<128, true, true>(a, stream);
     }

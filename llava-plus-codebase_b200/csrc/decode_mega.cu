@@ -41,12 +41,6 @@ constexpr int MK_TILE_BYTES = 8 * MK_ROW_STRIDE;
 constexpr int MK_MAXNB = 32;                  // max 8-row blocks per CTA per phase (host-checked)
 constexpr int MK_MAXL = 48;                   // decoder layers whose weight-pointer table is cached in smem
 constexpr int MK_MAX_STAGES = 12;
-// L2 look-ahead (MegaParams::l2_ahead tiles, l2_mode): the producer that issues the ring load of tile t also pulls
-// tile t + l2_ahead of its own sequence into L2, so L2 (50 MB on the H100) extends the ring: HBM keeps streaming for
-// (stages + l2_ahead) tiles while the consumers sit in a dependency, and the ring refills from L2 hits afterwards.
-//   mode 1: prefetch.global.L2 per 128 B line from the LSU (does not queue in front of the TMA ring loads)
-//   mode 2: cp.async.bulk.prefetch.L2 per row piece (TMA queue). The ring loads queue behind these prefetches in the TMA engine.
-// Off by default (model.cu); not measured on the H100.
 
 __device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
     f[0] = bf16_lo(u.x); f[1] = bf16_hi(u.x); f[2] = bf16_lo(u.y); f[3] = bf16_hi(u.y);
@@ -209,108 +203,6 @@ __device__ __forceinline__ void mk_prologue(const PhaseIO& c, int K, int B, floa
         }
     }
     cons_sync();
-}
-
-// Single-pass variant (MegaParams::fast_prologue): every load of the phase's activation vector is issued before the
-// first use (one L2 round trip instead of one per loop iteration), the RMSNorm weights arrive in registers (`gpre`,
-// loaded BEFORE the grid barrier: they do not depend on activations), and each thread sums the 16 warp partials
-// itself (one CTA barrier fewer). Same summation order -> bit-identical to mk_prologue. Needs K/8 <= 2*MK_CONS when
-// gamma is set (the caller checks).
-template <int NB>
-__device__ __forceinline__ void mk_prologue_fast(const PhaseIO& c, int K, float eps, int tid, int lane, int warp,
-                                                 __nv_bfloat16* xs, float (*s_red)[NB], const uint4 (&gpre)[2]) {
-    const int nvec = K >> 3;
-    if (c.gamma == nullptr) {
-        constexpr int J = 3;
-        for (int i0 = 0; i0 < nvec; i0 += J * MK_CONS) {
-            uint4 u[NB][J];
-#pragma unroll
-            for (int j = 0; j < J; ++j) {
-                const int idx = i0 + j * MK_CONS + tid;
-#pragma unroll
-                for (int b = 0; b < NB; ++b)
-                    u[b][j] = idx < nvec ? ldcg16(c.xin + (size_t)b * K + idx * 8) : make_uint4(0, 0, 0, 0);
-            }
-#pragma unroll
-            for (int j = 0; j < J; ++j) {
-                const int idx = i0 + j * MK_CONS + tid;
-                if (idx < nvec) {
-#pragma unroll
-                    for (int b = 0; b < NB; ++b) *reinterpret_cast<uint4*>(xs + (size_t)b * K + idx * 8) = u[b][j];
-                }
-            }
-        }
-        cons_sync();
-        return;
-    }
-    uint4 u[NB][2];
-    float ss[NB];
-#pragma unroll
-    for (int b = 0; b < NB; ++b) ss[b] = 0.f;
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-        const int idx = j * MK_CONS + tid;
-#pragma unroll
-        for (int b = 0; b < NB; ++b)
-            u[b][j] = idx < nvec ? ldcg16(c.xin + (size_t)b * K + idx * 8) : make_uint4(0, 0, 0, 0);
-    }
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-#pragma unroll
-        for (int b = 0; b < NB; ++b) {
-            float f[8];
-            unpack8(u[b][j], f);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) ss[b] += f[e] * f[e];
-        }
-    }
-#pragma unroll
-    for (int b = 0; b < NB; ++b) {
-        const float v = warp_sum(ss[b]);
-        if (lane == 0) s_red[warp][b] = v;
-    }
-    cons_sync();
-    float rstd[NB];
-#pragma unroll
-    for (int b = 0; b < NB; ++b) {
-        float t = 0.f;
-#pragma unroll
-        for (int i = 0; i < MK_CONS_WARPS; ++i) t += s_red[i][b];
-        rstd[b] = rsqrtf(t / K + eps);
-    }
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-        const int idx = j * MK_CONS + tid;
-        if (idx < nvec) {
-            float gf[8];
-            unpack8(gpre[j], gf);
-#pragma unroll
-            for (int b = 0; b < NB; ++b) {
-                float f[8], o[8];
-                unpack8(u[b][j], f);
-#pragma unroll
-                for (int e = 0; e < 8; ++e) o[e] = gf[e] * round_bf16(f[e] * rstd[b]);
-                *reinterpret_cast<uint4*>(xs + (size_t)b * K + idx * 8) =
-                    make_uint4(pack_bf16(o[0], o[1]), pack_bf16(o[2], o[3]), pack_bf16(o[4], o[5]), pack_bf16(o[6], o[7]));
-            }
-        }
-    }
-    cons_sync();  // xs complete; also orders the s_red reads above before the next phase's writes
-}
-
-// RMSNorm weights of GEMV phase `ph` into registers (independent of activations: issued before the grid barrier)
-__device__ __forceinline__ bool mk_gamma_preload(const MegaParams& p, const MegaLayer* layers, int ph, int n_phases,
-                                                 int tid, uint4 (&gpre)[2]) {
-    if (ph >= n_phases || mk_is_attention(p, ph)) return false;
-    const PhaseIO io = mk_phase_io(p, layers, ph);
-    const int nvec = p.h >> 3;  // every normed phase has K = h
-    if (io.gamma == nullptr || nvec > 2 * MK_CONS) return false;
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-        const int idx = j * MK_CONS + tid;
-        gpre[j] = idx < nvec ? __ldg(reinterpret_cast<const uint4*>(io.gamma) + idx) : make_uint4(0, 0, 0, 0);
-    }
-    return true;
 }
 
 __device__ __forceinline__ void mk_mma(float (&c)[4], uint32_t a0, uint32_t a2, uint32_t b0, uint32_t b1) {
@@ -555,13 +447,6 @@ __device__ __forceinline__ void cursor_next(TileCursor& t, const MegaParams& p, 
     ++t.ph;
     cursor_seek(t, p, layers, n_phases);
 }
-__device__ __forceinline__ void prefetch_l2_line(const void* gsrc) {
-    asm volatile("prefetch.global.L2 [%0];" ::"l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void bulk_prefetch_l2(const void* gsrc, uint32_t bytes) {
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gsrc), "r"(bytes) : "memory");
-}
-
 template <int NB>
 __global__ void __launch_bounds__(MK_THREADS, 1) decode_mega_kernel(MegaParams p, int n_stages) {
     extern __shared__ __align__(128) uint8_t mk_smem[];
@@ -601,37 +486,12 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_mega_kernel(MegaParams p
 
     if (warp >= MK_CONS_WARPS) {
         // =========================== PRODUCERS: stream every phase's weight tiles, in order ===========================
-        // `cp` feeds the shared-memory ring with TMA bulk copies, throttled by free ring slots; `pf` runs l2_ahead
-        // tiles in front of it and only touches L2 (see the note at MK_L2 above).
+        // `cp` feeds the shared-memory ring with TMA bulk copies, throttled by free ring slots
         const uint32_t pw = (uint32_t)(warp - MK_CONS_WARPS);
-        const uint32_t ahead = (uint32_t)p.l2_ahead;  // multiple of MK_PROD_WARPS: pf stays in this warp's residue class
-        TileCursor cp, pf;
+        TileCursor cp;
         cursor_begin(cp, p, s_layers, n_phases);
-        cursor_begin(pf, p, s_layers, n_phases);
         while (cp.valid) {
             if (cp.tile % (uint32_t)MK_PROD_WARPS == pw) {
-                if (ahead != 0) {
-                    // L2 look-ahead first, so it is already in flight while this warp waits for a free ring slot
-                    while (pf.valid && pf.tile < cp.tile + ahead) cursor_next(pf, p, s_layers, n_phases);
-                    if (pf.valid) {
-                        const uint32_t pbytes = (uint32_t)min(MK_KT, pf.c.K - pf.kc * MK_KT) * 2u;
-                        if (p.l2_mode == 2) {
-                            bool pvalid;
-                            const int pfrow = mk_phys_row(pf.c, pf.rb, lane & 7, pvalid);
-                            if (lane < 8 && pvalid)
-                                bulk_prefetch_l2(pf.c.W + (size_t)pfrow * pf.c.K + (size_t)pf.kc * MK_KT, pbytes);
-                        } else {
-                            bool pvalid;  // 4 lanes per row, 128 B lines dealt round-robin
-                            const int pfrow = mk_phys_row(pf.c, pf.rb, lane >> 2, pvalid);
-                            if (pvalid) {
-                                const char* base = reinterpret_cast<const char*>(pf.c.W + (size_t)pfrow * pf.c.K +
-                                                                                 (size_t)pf.kc * MK_KT);
-                                for (uint32_t off = (uint32_t)(lane & 3) * 128u; off < pbytes; off += 512u)
-                                    prefetch_l2_line(base + off);
-                            }
-                        }
-                    }
-                }
                 const uint32_t stage = cp.tile % (uint32_t)n_stages;
                 const uint32_t parity = (cp.tile / (uint32_t)n_stages) & 1u;
                 const uint32_t row_bytes = (uint32_t)min(MK_KT, cp.c.K - cp.kc * MK_KT) * 2u;
@@ -668,13 +528,11 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_mega_kernel(MegaParams p
         uint4* dst = reinterpret_cast<uint4*>(p.x + (size_t)blockIdx.x * p.h);
         for (int i = tid; i < p.h / 8; i += MK_CONS) dst[i] = src[i];
     }
-    uint4 gpre[2] = {make_uint4(0, 0, 0, 0), make_uint4(0, 0, 0, 0)};
-    bool gpre_ok = p.fast_prologue != 0 && mk_gamma_preload(p, s_layers, 0, n_phases, tid, gpre);
-    // gamma_smem knob: the RMSNorm weights of the NEXT phase are copied (cp.async, no registers held) into the part of the
+    // The RMSNorm weights of the NEXT phase are copied (cp.async, no registers held) into the part of the
     // activation tile that a K = h phase leaves unused, in front of the grid barrier; the prologue then finds them in shared
     // memory instead of paying an L2/HBM round trip between its two passes.
     __nv_bfloat16* gsm = xs + (size_t)NB * p.h;
-    const bool gsm_fits = p.gamma_smem != 0 && (size_t)(NB + 1) * p.h <= (size_t)NB * (p.h > p.I ? p.h : p.I);
+    const bool gsm_fits = (size_t)(NB + 1) * p.h <= (size_t)NB * (p.h > p.I ? p.h : p.I);
     auto gamma_prefetch = [&](int ph) -> bool {
         if (!gsm_fits || ph >= n_phases || mk_is_attention(p, ph)) return false;
         const PhaseIO io = mk_phase_io(p, s_layers, ph);
@@ -706,10 +564,7 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_mega_kernel(MegaParams p
                 const int b = tid / c.nu, r = tid - b * c.nu;
                 res_pref = __bfloat162float(__ldcg(io.residual + (size_t)b * io.ld_out + (size_t)c.u_lo + r));
             }
-            if (p.fast_prologue != 0 && (io.gamma == nullptr || gpre_ok))
-                mk_prologue_fast<NB>(io, c.K, p.eps, tid, lane, warp, xs, s_red, gpre);
-            else
-                mk_prologue<NB>(io, c.K, B, p.eps, tid, lane, warp, xs, s_red, s_rstd, gsm_ok ? gsm : nullptr);
+            mk_prologue<NB>(io, c.K, B, p.eps, tid, lane, warp, xs, s_red, s_rstd, gsm_ok ? gsm : nullptr);
             if (tracing) p.trace[ph * 4 + 1] = clock64();
 #pragma unroll 1
             for (int rb = 0; rb < c.nb; ++rb) {
@@ -743,7 +598,6 @@ __global__ void __launch_bounds__(MK_THREADS, 1) decode_mega_kernel(MegaParams p
             mk_epilogue<NB>(p, s_layers, ph, c, B, tid, s_gpart, res_pref, have_res);
         }
         if (tracing) p.trace[ph * 4 + 3] = clock64();
-        gpre_ok = p.fast_prologue != 0 && mk_gamma_preload(p, s_layers, ph + 1, n_phases, tid, gpre);
         gsm_ok = gamma_prefetch(ph + 1);
         bar_target += gridDim.x;
         grid_sync(p.bar_count, bar_target);

@@ -67,7 +67,7 @@ struct SkEpi {
     int ld_out, ld_res, out_fp32, maxseg;
     const float* w_scale;           // fp8 only: [N] per weight row (physical row order of W)
     const float* x_scale;           // fp8 only: [B] per token
-    int stages;                     // ring depth actually used (<= SkCfg::STAGES); B2_SKINNY_STAGES
+    int stages;                     // ring depth: SkCfg<BN>::STAGES (set by sk_launch)
     unsigned long long* trace;      // debug (B2_SKINNY_TRACE=<file>): 16 slots (8 %globaltimer stamps + tiles finalised) per CTA of this launch, else nullptr
 };
 
@@ -403,7 +403,7 @@ SkPlan sk_plan(int B, int N, int K, bool fp8 = false) {
 }
 
 template <int BN, int ACT, bool FP8>
-int sk_launch(const CUtensorMap& tw, const CUtensorMap& tx, const SkPlan& pl, int N, int K, int B, const SkEpi& ep,
+int sk_launch(const CUtensorMap& tw, const CUtensorMap& tx, const SkPlan& pl, int N, int K, int B, SkEpi ep,
               cudaStream_t st) {
     using Cfg = SkCfg<BN>;
     static bool attr_set = false;
@@ -412,8 +412,8 @@ int sk_launch(const CUtensorMap& tw, const CUtensorMap& tx, const SkPlan& pl, in
         B2_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
         attr_set = true;
     }
-    const size_t smem = (size_t)ep.stages * Cfg::STAGE + Cfg::ACC_BYTES + Cfg::UP_BYTES + 1024 + 256;
-    B2_CUDA_CHECK(launch_pdl(kern, dim3(pl.grid), dim3(SK_THREADS), smem, st, tw, tx, N, K, B, ep));
+    ep.stages = Cfg::STAGES;
+    B2_CUDA_CHECK(launch_pdl(kern, dim3(pl.grid), dim3(SK_THREADS), (size_t)Cfg::SMEM, st, tw, tx, N, K, B, ep));
     B2_LAUNCH_CHECK();
     return 0;
 }
@@ -505,13 +505,6 @@ static int gemm_skinny_any(const SkinnyArgs& g, cudaStream_t stream) {
     ep.out = g.out; ep.partial = g.partial; ep.counters = g.counters;
     ep.ld_out = g.ld_out; ep.ld_res = g.ld_res; ep.out_fp32 = g.out_fp32; ep.maxseg = pl.maxseg;
     ep.w_scale = g.w_scale; ep.x_scale = g.x_scale;
-    {   // ring depth: the full ring by default; a shallower ring (<= half of the SM's shared memory) lets the CTAs of two
-        // consecutive launches share an SM under programmatic dependent launch. Re-read per launch (A/B inside one process).
-        const int full = pl.bn == 32 ? SkCfg<32>::STAGES : (pl.bn == 64 ? SkCfg<64>::STAGES : SkCfg<128>::STAGES);
-        const char* e = getenv("B2_SKINNY_STAGES");
-        const int want = e ? atoi(e) : 0;
-        ep.stages = (want >= 2 && want < full) ? want : full;
-    }
     ep.trace = sk_trace_slot(g.N, g.K, g.B, pl.grid, stream);
     const bool sw = g.act == ACT_SWIGLU;
     switch (pl.bn) {

@@ -582,7 +582,7 @@ cudaError_t launch_cluster_pdl(void (*kernel)(KArgs...), int grid, int cluster, 
     cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kNumThreads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
     cudaLaunchAttribute attr[2];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
     attr[1].id = cudaLaunchAttributeClusterDimension;
     attr[1].val.clusterDim.x = cluster; attr[1].val.clusterDim.y = 1; attr[1].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = cluster > 1 ? 2 : 1;

@@ -121,7 +121,7 @@ int vit_embed_ln(const void* patch_out, const void* cls, const void* pos, const 
 // out[b, p, :] = hidden[b, 1 + p, :]   (feature_select 'patch': drop CLS)
 int vit_drop_cls(const void* hidden, void* out, int B, int P, int D, cudaStream_t stream);
 
-// ---- attention (attention.cu) ----------------------------------------------------------------------
+// ---- attention (attention_wgmma.cu, attention.cu) ---------------------------------------------------
 struct FlashArgs {
     const void* q = nullptr; int64_t q_bs = 0, q_ts = 0, q_hs = 0;  // element strides: batch, token, head
     const void* k = nullptr; int64_t k_bs = 0, k_ts = 0, k_hs = 0;
@@ -129,16 +129,14 @@ struct FlashArgs {
     void* o = nullptr;       int64_t o_bs = 0, o_ts = 0, o_hs = 0;
     const int32_t* seq_lens = nullptr;  // device [B] or null (=S)
     // device [B] or null: query row t of sample b sits at absolute position pos0[b] + t and attends keys 0 .. pos0[b] + t of
-    // k / v, which then hold Skv rows per (b, head) (a KV cache). Causal, D = 128, wgmma kernel only.
+    // k / v, which then hold Skv rows per (b, head) (a KV cache). Causal, D = 128.
     const int32_t* pos0 = nullptr;
     int Skv = 0;
     int B = 0, H = 0, S = 0, D = 0;     // S = padded/query length; D in {64, 128}
     int causal = 0;
     float scale = 1.f;
 };
-int flash_attn_bf16(const FlashArgs& a, cudaStream_t stream);      // dispatcher (wgmma unless B2_FLASH_TC=0)
-int flash_attn_tc_bf16(const FlashArgs& a, cudaStream_t stream);   // attention_wgmma.cu: wgmma + TMA
-int flash_attn_mma_bf16(const FlashArgs& a, cudaStream_t stream);  // attention.cu: mma.sync variant
+int flash_attn_bf16(const FlashArgs& a, cudaStream_t stream);  // attention_wgmma.cu: wgmma + TMA
 
 // prefill: RoPE on q (in place) and k inside qkv [B*S, 3*H*D]; roped k and v written to the cache
 // kcache/vcache: [Bmax, H, Smax, D] for one layer. Positions are 0..S-1 (right-padded rows).
@@ -204,10 +202,6 @@ struct MegaParams {
     unsigned int *bar_count = nullptr, *done_count = nullptr;  // zero-initialised
     unsigned int bar_base = 0;  // barrier-counter value before this launch = launches so far * (5L+2) * grid
     float eps = 1e-5f, theta = 10000.f, scale_log2 = 1.f;
-    int l2_ahead = 0;       // weight tiles pulled into L2 in front of the shared-memory ring (0 = off), multiple of 4
-    int l2_mode = 1;        // 1 = prefetch.global.L2 lines (LSU), 2 = cp.async.bulk.prefetch.L2 (TMA queue)
-    int fast_prologue = 0;  // single-pass activation staging with pre-barrier RMSNorm-weight loads
-    int gamma_smem = 0;     // next phase's RMSNorm weights staged in shared memory (cp.async) in front of the grid barrier
     long long* trace = nullptr;  // optional [n_phases+2][4] SM-clock timestamps of CTA 0 (B2_MEGA_TRACE=<file>)
     // token publication to the host ring (sampling.cu): non-null only for greedy streaming; with do_sample the separate
     // sample_publish kernel that follows the launch overrides the fused argmax and publishes instead

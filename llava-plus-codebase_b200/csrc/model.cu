@@ -25,11 +25,6 @@ namespace b2 {
 static thread_local char g_err[1024] = {0};
 unsigned long long g_launch_count = 0;
 
-bool pdl_enabled() {  // read per launch (one getenv) so that one process can A/B it; graphs keep what they were captured with
-    const char* e = getenv("B2_PDL");
-    return !(e != nullptr && e[0] == '0');
-}
-
 void set_error(const char* fmt, ...) {
     va_list ap;
     va_start(ap, fmt);
@@ -388,8 +383,6 @@ int decode_nsplit(int B, int H, int max_seq, int ctas_per_sm) {
     // Split-KV factor of the multi-kernel decode step. The kernel is register-limited to `occ` resident CTAs per SM, so one wave
     // is occ*SMs CTAs. Few (batch, head) pairs: fill one wave; otherwise 3 splits (short enough ranges for the tail wave to
     // overlap, few enough partials for the merge to stay cheap).
-    const char* e = getenv("B2_DECODE_NSPLIT");
-    if (e != nullptr && atoi(e) >= 1) return atoi(e) > 32 ? 32 : atoi(e);
     const int cap = ctas_per_sm * num_sms();
     int n = cap / (B * H);
     if (n < 3) n = 3;
@@ -556,15 +549,9 @@ int project_rows(b2_model* m, const void* feats, int rows, void* out, cudaStream
         const int n = rows - r0 < max_rows ? rows - r0 : max_rows;
         const bf16* a = reinterpret_cast<const bf16*>(feats) + (size_t)r0 * D;
         bf16* o = reinterpret_cast<bf16*>(out) + (size_t)r0 * h;
-        const char* pf = getenv("B2_PROJECTOR_FUSED");  // =0 restores the two-launch form (A/B runs, read per call)
-        if (!(pf != nullptr && pf[0] == '0')) {
-            // north_star: "mm_projector as one fused GEMM->GELU->GEMM kernel" (phase-2 tiles gated on per-row-block counters)
-            B2_TRY(projector_fused_bf16(a, D, m->p0_w.p, m->p0_b.p, m->p2_w.p, m->p2_b.p, m->p_mid.p, o, h, n, D, h, h,
-                                        m->p_done.as<int>(), st));
-        } else {
-            B2_TRY(gemm(a, D, m->p0_w.p, D, m->p0_b.p, nullptr, 0, m->p_mid.p, h, 0, n, h, D, ACT_GELU_ERF, st));
-            B2_TRY(gemm(m->p_mid.p, h, m->p2_w.p, h, m->p2_b.p, nullptr, 0, o, h, 0, n, h, h, ACT_NONE, st));
-        }
+        // north_star: "mm_projector as one fused GEMM->GELU->GEMM kernel" (phase-2 tiles gated on per-row-block counters)
+        B2_TRY(projector_fused_bf16(a, D, m->p0_w.p, m->p0_b.p, m->p2_w.p, m->p2_b.p, m->p_mid.p, o, h, n, D, h, h,
+                                    m->p_done.as<int>(), st));
     }
     return 0;
 }
@@ -592,11 +579,6 @@ int capture_graph(cudaStream_t st, cudaGraphExec_t* exec, int* launches, F fn) {
 // eagerly (function attributes, driver entry points), the second captures, later ones replay.
 int encode_chunk(b2_model* m, const void* pixels, int n, void* out, cudaStream_t st) {
     const b2_model_desc& d = m->d;
-    const char* eg = getenv("B2_ENCODE_GRAPH");  // =0: launch by launch (A/B runs)
-    if (eg != nullptr && eg[0] == '0') {
-        B2_TRY(vit_forward_chunk(m, pixels, n, m->v_feats.p, st));
-        return project_rows(m, m->v_feats.p, n * m->P, out, st);
-    }
     const size_t in_bytes = (size_t)n * 3 * d.image_size * d.image_size * 2, out_bytes = (size_t)n * m->P * d.hidden * 2;
     cudaStream_t run = st;
     if (st == nullptr || st == cudaStreamLegacy) {
@@ -709,11 +691,6 @@ bool use_mega(const b2_model* m, const b2_kv* kv, int B) {
     return flag == 1;
 }
 
-// defaults of the megakernel knobs: both off; neither has been measured on the H100 (its L2 is 50 MB, so the look-ahead has
-// less room than the knob was written for)
-constexpr int kMegaL2AheadDefault = 0;
-constexpr int kMegaFastPrologueDefault = 0;
-
 int decode_step_mega(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     const b2_model_desc& d = m->d;
     MegaParams p;
@@ -738,17 +715,6 @@ int decode_step_mega(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     const bool sampling = kv->samp_host.do_sample != 0 || kv->samp_host.per_row != 0 || kv->any_proc();
     if (!sampling && kv->samp_host.tag != 0) { p.sstate = kv->sstate.as<SampleState>(); p.ring = kv->ring_dev; p.ring_cap = kv->ring_cap; }
     if (kv->samp_host.per_row) p.rows = kv->rows_dev.as<RowState>();
-    {   // tuning knobs, re-read every launch so a sweep can flip them inside one process (scripts/mega_sweep.py)
-        const char* e = getenv("B2_MEGA_L2_AHEAD");
-        int ahead = e ? atoi(e) : kMegaL2AheadDefault;
-        p.l2_ahead = ahead < 0 ? 0 : (ahead > 64 ? 64 : ahead) / 4 * 4;
-        e = getenv("B2_MEGA_L2_MODE");
-        p.l2_mode = (e && e[0] == '2') ? 2 : 1;
-        e = getenv("B2_MEGA_FAST_PROLOGUE");
-        p.fast_prologue = e ? (e[0] != '0') : kMegaFastPrologueDefault;
-        e = getenv("B2_MEGA_GAMMA_SMEM");
-        p.gamma_smem = e ? (e[0] != '0') : 1;
-    }
     static int trace_mode = -1;
     if (trace_mode < 0) { const char* e = getenv("B2_MEGA_TRACE"); trace_mode = (e && e[0] != 0) ? 1 : 0; }
     if (trace_mode == 1) {

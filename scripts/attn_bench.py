@@ -1,4 +1,4 @@
-"""Time b2_op_flash_attn (C-ABI) on the path's attention shapes, the wgmma and the mma.sync kernel in one process (B2_FLASH_TC is re-read per call).
+"""Time b2_op_flash_attn (C-ABI, the wgmma flash-attention kernel) on the path's attention shapes.
 
     python scripts/attn_bench.py            # prints one line per shape: us, TFLOP/s, max-abs-diff vs torch fp32
 """
@@ -22,9 +22,7 @@ def main():
     lib = _b2.load_library()
     _b2.check(lib.b2_init(0))
     dev = torch.device("cuda:0")
-    variants = [("wgmma", "1"), ("mma.sync", "0")]
-    for (tag, tc), (B, S, H, D, causal) in [(v, sh) for sh in SHAPES for v in variants]:
-        os.environ["B2_FLASH_TC"] = tc
+    for B, S, H, D, causal in SHAPES:
         g = torch.Generator(device=dev).manual_seed(1)
         q, k, v = (torch.randn(B, S, H, D, device=dev, generator=g).to(torch.bfloat16) for _ in range(3))
         o = torch.empty_like(q)
@@ -52,7 +50,7 @@ def main():
             s = s.masked_fill(torch.triu(torch.ones(S, S, device=dev, dtype=torch.bool), 1), float("-inf"))
         want = (torch.softmax(s, -1) @ vf).permute(1, 0, 2)
         err = (o[0, :, :4].float() - want).abs().max().item()
-        print(f"[{tag}] B={B} S={S} H={H} D={D} causal={causal}: {us:9.1f} us  {flops / us / 1e6:8.1f} TFLOP/s  "
+        print(f"B={B} S={S} H={H} D={D} causal={causal}: {us:9.1f} us  {flops / us / 1e6:8.1f} TFLOP/s  "
               f"max|err|={err:.4f}", flush=True)
 
 

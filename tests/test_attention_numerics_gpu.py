@@ -450,12 +450,10 @@ def _check_problems(kind, case, probs, out_of):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("tc", [1, 0], ids=["wgmma", "mma"])
-@pytest.mark.parametrize("case", FLASH_CASES, ids=[_cid(c) for c in FLASH_CASES])
-def test_flash_attn(lib, case, tc, monkeypatch):
+@pytest.mark.parametrize("case", FLASH_CASES, ids=[_cid(c) + "-wgmma" for c in FLASH_CASES])
+def test_flash_attn(lib, case):
     from llava import _b2
 
-    monkeypatch.setenv("B2_FLASH_TC", str(tc))  # the dispatcher re-reads it on every call
     inp, probs = build_flash(case, seed=1)
     B, S, H, D = case["B"], case["S"], case["H"], case["D"]
     q, k, v = (inp[n].to(DEV) for n in ("q", "k", "v"))
@@ -463,7 +461,7 @@ def test_flash_attn(lib, case, tc, monkeypatch):
     o = torch.full_like(q, float("nan"))
     _b2.check(lib.b2_op_flash_attn(_P(q), _P(k), _P(v), _P(o), _P(lens), B, S, H, D, case["causal"], D ** -0.5, _S()))
     o = o.cpu()
-    _check_problems("flash_" + ("wgmma" if tc else "mma"), case, probs, lambda b, h: o[b, :, h])
+    _check_problems("flash_wgmma", case, probs, lambda b, h: o[b, :, h])
 
 
 @pytest.mark.gpu

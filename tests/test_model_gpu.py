@@ -429,10 +429,25 @@ def test_rope_fused_into_qkv_gemm_equals_the_standalone_pass():
     eng.close()
 
 
+def _two_gemm_projector(w, feats):
+    """mm_projector as two b2_op_gemm launches (bias + erf GELU into a bf16 H, then bias): the GEMM the fused kernel runs."""
+    lib = _b2.load_library()
+    x = feats.reshape(-1, feats.shape[-1]).to(DEV)
+    W1, b1, W2, b2 = (w[f"model.mm_projector.{k}"].to(DEV, torch.bfloat16) for k in ("0.weight", "0.bias", "2.weight", "2.bias"))
+    (M, K), N = x.shape, W1.shape[0]
+    mid, out = (torch.empty(M, N, device=DEV, dtype=torch.bfloat16) for _ in range(2))
+    st = _b2.stream_ptr()
+    _b2.check(lib.b2_op_gemm(_b2.ptr(x), K, _b2.ptr(W1), K, _b2.ptr(b1), None, 0, _b2.ptr(mid), N, 0, M, N, K, _b2.ACT_GELU_ERF,
+                             0, st), "b2_op_gemm")
+    _b2.check(lib.b2_op_gemm(_b2.ptr(mid), N, _b2.ptr(W2), N, _b2.ptr(b2), None, 0, _b2.ptr(out), N, 0, M, N, N, _b2.ACT_NONE,
+                             0, st), "b2_op_gemm")
+    return out.reshape(*feats.shape[:-1], N)
+
+
 @pytest.mark.parametrize("n_img", [1, 3, 20])
 def test_fused_projector_kernel_equals_the_two_gemm_form(n_img):
     """north_star: "mm_projector as one fused GEMM->GELU->GEMM kernel". The single-launch kernel (phase-2 tiles gated on
-    per-row-block completion counters) against the two-launch form of the same GEMM (B2_PROJECTOR_FUSED=0) and the oracle,
+    per-row-block completion counters) against the two-launch form of the same GEMM (two b2_op_gemm calls) and the oracle,
     at the 7B projector shape; 20 images = 90 row blocks = 12 dependency groups, repeated to catch a stale read of H."""
     cfg = O.make_config(hidden=4096, inter=11008, layers=1, heads=32, vit_layers=2)
     w = O.make_weights(cfg, seed=21)
@@ -440,16 +455,11 @@ def test_fused_projector_kernel_equals_the_two_gemm_form(n_img):
     g = torch.Generator().manual_seed(n_img)
     feats = (torch.randn(n_img, 576, 1024, generator=g)).to(torch.bfloat16)
     ref = O.mm_projector(w, feats.float())
-    try:
-        os.environ["B2_PROJECTOR_FUSED"] = "0"
-        two = eng.project(feats.to(DEV)).float().cpu()
-        os.environ["B2_PROJECTOR_FUSED"] = "1"
-        for rep in range(4):
-            one = eng.project(feats.to(DEV)).float().cpu()
-            assert torch.isfinite(one).all()
-            # same operands, same fp32 accumulation order per output element (tile width may differ): <= 1 bf16 ulp apart
-            torch.testing.assert_close(one, two, rtol=2 ** -7, atol=1e-3)
-    finally:
-        os.environ.pop("B2_PROJECTOR_FUSED", None)
+    two = _two_gemm_projector(w, feats).float().cpu()
+    for rep in range(4):
+        one = eng.project(feats.to(DEV)).float().cpu()
+        assert torch.isfinite(one).all()
+        # same operands, same fp32 accumulation order per output element (tile width may differ): <= 1 bf16 ulp apart
+        torch.testing.assert_close(one, two, rtol=2 ** -7, atol=1e-3)
     _check(f"fused projector ({n_img} images)", one, ref)
     eng.close()

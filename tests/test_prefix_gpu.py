@@ -79,15 +79,6 @@ def test_flash_attn_kv_at_position_zero_is_the_plain_kernel(n):
         assert torch.equal(o1[b, :L], o2[b, :L]), b
 
 
-def test_flash_attn_kv_rejects_the_mma_fallback(monkeypatch):
-    lib = _b2.load_library()
-    t = torch.zeros(1 << 20, device=DEV, dtype=BF)
-    monkeypatch.setenv("B2_FLASH_TC", "0")
-    zero = i32([0])
-    assert lib.b2_op_flash_attn_kv(P(t), P(t), P(t), P(t), P(zero), None, 1, 16, 2, 256, 0.1, S()) == -1
-    assert "wgmma" in _b2.last_error()
-
-
 def test_rope_kv_write_at_equals_whole_sequence_rows():
     lib = _b2.load_library()
     B, H, n, Smax = 3, 32, 77, 1024
