@@ -234,6 +234,20 @@ int b2_stream_begin_ex(b2_model* m, b2_kv* kv, const float* logits, int B, const
                        void* stream);
 int b2_stream_enqueue(b2_model* m, b2_kv* kv, int n_steps, void* stream);
 int b2_stream_wait(b2_kv* kv, int index, int32_t* tokens_host, int timeout_ms);
+/* Score and logits rows of a streaming generation (generate(output_scores / output_logits, return_dict_in_generate)).
+ *   b2_stream_set_outputs  arms device fp32 buffers [cap_steps][B][vocab] (either nullable; both NULL disarms) for the next
+ *                          b2_stream_begin / b2_stream_begin_ex on this cache, which takes them over whether or not it succeeds.
+ *                          The step that publishes token t of that generation writes row t = [B][vocab] of each: `logits` gets
+ *                          the raw fp32 logits it selected from, `scores` the row HF hands to selection: the logits after the
+ *                          processors, and when sampling x / T (IEEE division) with the tokens the top-k / top-p filters remove
+ *                          at -inf. Token 0 is written by the begin, from the prefill logits. Steps queued past cap_steps write
+ *                          nothing. The buffers are written by every step of the generation on the stream the steps run on, so
+ *                          they must stay allocated until the steps queued for it have run (b2_stream_enqueue orders them before
+ *                          later work on the caller's stream) and until the next call that begins a generation or decodes on the
+ *                          cache (b2_stream_begin*, b2_batch_begin, b2_decode_step, b2_decode_greedy, b2_beam_step*). A finished
+ *                          row keeps decoding its own tokens, so its rows after its eos are not HF's. b2_stream_begin_lookup and
+ *                          b2_batch_begin return -1 while buffers are armed. */
+int b2_stream_set_outputs(b2_kv* kv, float* scores, float* logits, int cap_steps);
 
 /* Prompt-lookup speculative decoding of one sample (HF generate(prompt_lookup_num_tokens=K, max_matching_ngram_size=n): the draft is
  * copied from the conversation itself). Every step drafts up to K tokens from the history on the device (the prompt ids, then the
@@ -342,6 +356,20 @@ int b2_op_beam_sample(const float* logits, const int32_t* row_of_beam, const flo
                       void* stream);
 int b2_beam_step_ex(b2_model* m, b2_kv* kv, const b2_beam_step_args* args, const b2_beam_sampling* sampling, uint32_t step,
                     void* stream);
+/* Score and logits rows of beam search (generate(output_scores / output_logits, return_dict_in_generate) with num_beams > 1).
+ *   b2_op_beam_select_out  b2_op_beam_topk (sampling NULL) or b2_op_beam_sample that also writes, for every beam row
+ *                          i = b*nb + j it reads, its score row to row_scores[(i*fan + r) * vocab ...] and the raw logits row to
+ *                          row_logits[...] for r < fan (device fp32, either nullable). The score row is log_softmax of the logits
+ *                          (fp32, ((x - max) - lse)), under sampling warped as b2_op_beam_sample warps it, -inf outside the
+ *                          survivors. fan > 1 (1..32, greedy only) fills the nb running rows of a sample from its one prefill row
+ *                          (nb = 1, fan = num_beams), as HF's first step of beam search has nb equal rows.
+ *   b2_beam_step_out       b2_beam_step_ex that writes the step's rows, [B*nb][vocab] in running-beam order (beam i reads the
+ *                          logits of slot slot_of_beam_host[i]), to row_scores / row_logits (device, nullable). */
+int b2_op_beam_select_out(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
+                          const b2_beam_sampling* sampling, uint32_t step, int fan, float* out_scores, int32_t* out_tokens,
+                          int32_t* out_beams, float* row_scores, float* row_logits, void* stream);
+int b2_beam_step_out(b2_model* m, b2_kv* kv, const b2_beam_step_args* args, const b2_beam_sampling* sampling, uint32_t step,
+                     float* row_scores, float* row_logits, void* stream);
 
 /* ---- single-kernel entry points (unit-level parity tests; same kernels the hot path launches) ----------- */
 int b2_op_gemm(const void* A, int lda, const void* W, int ldw, const void* bias, const void* residual, int ld_res,

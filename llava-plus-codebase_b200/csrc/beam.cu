@@ -127,7 +127,7 @@ __device__ __forceinline__ void stage_row(const float* __restrict__ x, float* s_
 
 __global__ void __launch_bounds__(BT_THREADS, 1)
 beam_row_topk_kernel(const float* __restrict__ logits, const int32_t* __restrict__ row_of_beam, const float* __restrict__ beam_scores,
-                     int nb, int V, int K, unsigned long long* __restrict__ keys_out) {
+                     int nb, int V, int K, unsigned long long* __restrict__ keys_out, BeamRowsOut ro) {
     extern __shared__ __align__(16) uint8_t bt_smem[];
     float* s_x = reinterpret_cast<float*>(bt_smem);
     __shared__ RowSmem sm;
@@ -140,7 +140,15 @@ beam_row_topk_kernel(const float* __restrict__ logits, const int32_t* __restrict
     float mx, lse;
     stage_row(logits + (size_t)row * V, s_x, V, tid, sm, mx, lse);
     const float run = beam_scores[beam];
-    for (int i = tid; i < V; i += BT_THREADS) s_x[i] = ((s_x[i] - mx) - lse) + run;
+    const size_t out0 = (size_t)beam * ro.fan * V;
+    for (int i = tid; i < V; i += BT_THREADS) {
+        const float x = s_x[i], ls = (x - mx) - lse;
+        s_x[i] = ls + run;
+        for (int r = 0; r < ro.fan; ++r) {  // output rows: the log-softmax row and the raw row, once per running beam it feeds
+            if (ro.scores != nullptr) ro.scores[out0 + (size_t)r * V + i] = ls;
+            if (ro.logits != nullptr) ro.logits[out0 + (size_t)r * V + i] = x;
+        }
+    }
     __syncthreads();
     row_top_candidates(s_x, V, Kr, (unsigned long long)j * V, tid, sm);
 
@@ -164,7 +172,7 @@ beam_row_topk_kernel(const float* __restrict__ logits, const int32_t* __restrict
 __global__ void __launch_bounds__(BT_THREADS, 1)
 beam_row_sample_kernel(const float* __restrict__ logits, const int32_t* __restrict__ row_of_beam, const float* __restrict__ beam_scores,
                        int nb, int V, int K, BeamSampleParams sp, unsigned long long* __restrict__ keys_out,
-                       float* __restrict__ scores_out) {
+                       float* __restrict__ scores_out, BeamRowsOut ro) {
     extern __shared__ __align__(16) uint8_t bt_smem[];
     float* s_x = reinterpret_cast<float*>(bt_smem);
     __shared__ RowSmem sm;
@@ -179,7 +187,11 @@ beam_row_sample_kernel(const float* __restrict__ logits, const int32_t* __restri
 
     float mx, lse;
     stage_row(x, s_x, V, tid, sm, mx, lse);
-    for (int i = tid; i < V; i += BT_THREADS) s_x[i] = __fdiv_rn((s_x[i] - mx) - lse, T);
+    const size_t out0 = (size_t)beam * V;  // beam sampling reads one row per running beam: fan is 1
+    for (int i = tid; i < V; i += BT_THREADS) {
+        if (ro.logits != nullptr) ro.logits[out0 + i] = s_x[i];
+        s_x[i] = __fdiv_rn((s_x[i] - mx) - lse, T);
+    }
     __syncthreads();
 
     // top-k: keep w >= the k-th largest w (ties kept), k = max(top_k, min_keep)
@@ -225,6 +237,7 @@ beam_row_sample_kernel(const float* __restrict__ logits, const int32_t* __restri
     const uint32_t flat_base = (uint32_t)beam * (uint32_t)V;
     for (int i = tid; i < V; i += BT_THREADS) {
         const float w = s_x[i];
+        if (ro.scores != nullptr) ro.scores[out0 + i] = w;  // the warped row, -inf outside the survivors
         if (w == w && w > -INFINITY) {
             const float acc = w + run;
             const unsigned long long r = philox_u64(sp.seed, sp.step, flat_base + (uint32_t)i);
@@ -307,8 +320,10 @@ kv_copy_slots_kernel(uint8_t* __restrict__ k, uint8_t* __restrict__ v, float* __
 size_t beam_topk_workspace_bytes(int B, int nb, int K) { return (size_t)B * nb * K * sizeof(unsigned long long); }
 
 int beam_topk(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
-              void* workspace, float* out_scores, int32_t* out_tokens, int32_t* out_beams, cudaStream_t stream) {
+              void* workspace, float* out_scores, int32_t* out_tokens, int32_t* out_beams, cudaStream_t stream,
+              const BeamRowsOut& rows_out) {
     B2_CHECK_ARG(logits && beam_scores && workspace && out_scores && out_tokens && out_beams, "beam_topk: null argument");
+    B2_CHECK_ARG(rows_out.fan >= 1, "beam_topk: %d output rows per beam", rows_out.fan);
     B2_CHECK_ARG(B >= 1 && nb >= 1 && nb <= 32, "beam_topk: B=%d nb=%d (1 <= nb <= 32)", B, nb);
     B2_CHECK_ARG(K >= 1 && K <= 128 && (long long)K <= (long long)nb * V, "beam_topk: K=%d outside [1, min(128, nb*V=%lld)]", K,
                  (long long)nb * V);
@@ -321,7 +336,7 @@ int beam_topk(const float* logits, const int32_t* row_of_beam, const float* beam
         attr = smem;
     }
     auto* keys = reinterpret_cast<unsigned long long*>(workspace);
-    beam_row_topk_kernel<<<dim3(nb, B), BT_THREADS, smem, stream>>>(logits, row_of_beam, beam_scores, nb, V, K, keys);
+    beam_row_topk_kernel<<<dim3(nb, B), BT_THREADS, smem, stream>>>(logits, row_of_beam, beam_scores, nb, V, K, keys, rows_out);
     B2_LAUNCH_CHECK();
     beam_merge_kernel<<<B, BM_THREADS, 0, stream>>>(keys, nullptr, nb, K, V, out_scores, out_tokens, out_beams);
     B2_LAUNCH_CHECK();
@@ -334,8 +349,9 @@ size_t beam_sample_workspace_bytes(int B, int nb, int K) {
 
 int beam_sample(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
                 const BeamSampleParams& sp, void* workspace, float* out_scores, int32_t* out_tokens, int32_t* out_beams,
-                cudaStream_t stream) {
+                cudaStream_t stream, const BeamRowsOut& rows_out) {
     B2_CHECK_ARG(logits && beam_scores && workspace && out_scores && out_tokens && out_beams, "beam_sample: null argument");
+    B2_CHECK_ARG(rows_out.fan == 1, "beam_sample: output rows are written once per beam row (fan %d)", rows_out.fan);
     B2_CHECK_ARG(B >= 1 && nb >= 1 && nb <= 32, "beam_sample: B=%d nb=%d (1 <= nb <= 32)", B, nb);
     B2_CHECK_ARG(K >= 1 && K <= 128 && (long long)K <= (long long)nb * V, "beam_sample: K=%d outside [1, min(128, nb*V=%lld)]", K,
                  (long long)nb * V);
@@ -353,7 +369,8 @@ int beam_sample(const float* logits, const int32_t* row_of_beam, const float* be
     }
     auto* keys = reinterpret_cast<unsigned long long*>(workspace);
     float* scores = reinterpret_cast<float*>(keys + (size_t)B * nb * K);
-    beam_row_sample_kernel<<<dim3(nb, B), BT_THREADS, smem, stream>>>(logits, row_of_beam, beam_scores, nb, V, K, sp, keys, scores);
+    beam_row_sample_kernel<<<dim3(nb, B), BT_THREADS, smem, stream>>>(logits, row_of_beam, beam_scores, nb, V, K, sp, keys, scores,
+                                                                        rows_out);
     B2_LAUNCH_CHECK();
     beam_merge_kernel<<<B, BM_THREADS, 0, stream>>>(keys, scores, nb, K, V, out_scores, out_tokens, out_beams);
     B2_LAUNCH_CHECK();

@@ -226,6 +226,11 @@ struct SampleState {
     int pub_counter;          // index of the next token of this generation
     unsigned int done;        // rows finished in the current launch (self-resetting)
     int per_row;              // continuous batching: selection parameters and liveness come from RowState[b] instead
+    // generate(output_scores / output_logits): fp32 rows [out_cap][B][V] (nullable). The step that publishes token t writes
+    // row t of each: the processed row it selected from (scores) and the raw logits it read (logits); t >= out_cap is skipped
+    float* out_scores;
+    float* out_logits;
+    int out_cap;
 };
 // One cache slot of a continuously batched decode (llava/_b2/batching.py): requests join and leave between steps, each with
 // its own sampling parameters and its own Philox draw index; a slot that is not active keeps its cache length and token.
@@ -292,6 +297,10 @@ int sample_state_set(SampleState* st_dev, const SampleState& v, cudaStream_t str
 int sample_publish(const float* logits, int V, int B, SampleState* st_dev, RowState* rows_dev, int32_t* tok, int32_t* out_tokens,
                    int32_t* step_counter, int32_t* cur_len, int32_t* ring_dev, int ring_cap, int flags, int step_offset,
                    const ProcState& proc, float* processed_out, cudaStream_t stream, SpecState* spec = nullptr);
+// the output rows of the step whose token the decode megakernel's fused argmax has just published (token pub_counter - 1): the
+// raw logits [B, V] to st->out_scores and st->out_logits (greedy without processors: the score row is the logits row). Selects
+// nothing, publishes nothing and leaves the counters alone.
+int publish_rows(const float* logits, int V, int B, const SampleState* st_dev, cudaStream_t stream);
 // row := v, its history := ids[0, len) (int64, device) followed by `first_token` when >= 0, and its bitmap rebuilt from those ids
 int proc_seed(const ProcState& proc, int row, const ProcRow& v, const int64_t* ids, int len, int first_token, int V,
               cudaStream_t stream);
@@ -302,8 +311,17 @@ int row_state_set(RowState* row_dev, const RowState& v, int32_t* tok_dev, int to
 // over its nb beams x V tokens, sorted by score descending, ties to the lower beam * V + token; row_of_beam null = identity.
 // nb <= 32, K <= min(128, nb * V); workspace >= beam_topk_workspace_bytes(B, nb, K)
 size_t beam_topk_workspace_bytes(int B, int nb, int K);
+// generate(output_scores / output_logits) of beam search: each beam row b*nb + j also writes its score row (log_softmax, warped
+// under beam sampling) to scores[(b*nb + j) * fan + r] and the raw logits it read to logits[...], r < fan, fp32 [V] each (both
+// nullable). fan > 1 fills the nb running rows of a sample from its one prefill row (the first step of beam search, nb = 1).
+struct BeamRowsOut {
+    float* scores = nullptr;
+    float* logits = nullptr;
+    int fan = 1;
+};
 int beam_topk(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
-              void* workspace, float* out_scores, int32_t* out_tokens, int32_t* out_beams, cudaStream_t stream);
+              void* workspace, float* out_scores, int32_t* out_tokens, int32_t* out_beams, cudaStream_t stream,
+              const BeamRowsOut& rows_out = BeamRowsOut{});
 // beam sampling: the same selection over Gumbel-perturbed keys of the warped scores (beam_row_sample_kernel in beam.cu); each
 // candidate's score is its unperturbed accumulated score. T > 0, top_k >= 0 (0 = off), top_p in (0, 1], min_keep >= 1.
 struct BeamSampleParams {
@@ -317,7 +335,7 @@ struct BeamSampleParams {
 size_t beam_sample_workspace_bytes(int B, int nb, int K);
 int beam_sample(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
                 const BeamSampleParams& sp, void* workspace, float* out_scores, int32_t* out_tokens, int32_t* out_beams,
-                cudaStream_t stream);
+                cudaStream_t stream, const BeamRowsOut& rows_out = BeamRowsOut{});
 struct KvCopyPairs {
     static constexpr int kMax = 64;
     int32_t src[kMax], dst[kMax], end[kMax];

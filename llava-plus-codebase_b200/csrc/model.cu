@@ -172,6 +172,10 @@ struct b2_kv {
     int ring_cap = 0;
     int epoch = 0;                 // generations started on this cache (tag = 1 + epoch % 2047)
     int stream_B = 0, stream_tag = 0, stream_scheduled = 0;  // streaming generation in progress: tokens scheduled so far
+    // output rows armed by b2_stream_set_outputs for the next b2_stream_begin(_ex), which takes them over (SampleState::out_*)
+    float* next_scores = nullptr;
+    float* next_logits = nullptr;
+    int next_cap = 0;
     DevBuf rows_dev;               // RowState[max_batch] (continuous batching)
     std::vector<RowState> rows_host;
     // b2_beam_step (allocated by the first call): beam -> slot map and running scores [2][max_batch], the per-row candidate
@@ -742,6 +746,9 @@ int decode_step_mega(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
         }
     }
     B2_TRY(decode_mega(p, st));
+    // output rows of the token the fused argmax published (the sampling launch below writes its own)
+    if (!sampling && p.ring != nullptr && kv->samp_host.out_cap > 0)
+        B2_TRY(publish_rows(m->logits.as<float>(), d.vocab, B, kv->sstate.as<SampleState>(), st));
     if (sampling)
         B2_TRY(sample_publish(m->logits.as<float>(), d.vocab, B, kv->sstate.as<SampleState>(), kv->rows_dev.as<RowState>(), kv->tok.as<int32_t>(),
                               kv->out_tokens.as<int32_t>(), kv->step_counter.as<int32_t>(), kv->len_dev.as<int32_t>(),
@@ -879,7 +886,7 @@ int b2_init(int device) {
 }
 
 const char* b2_last_error(void) { return g_err; }
-int b2_version(void) { return 8; }
+int b2_version(void) { return 9; }
 unsigned long long b2_launch_count(void) { return g_launch_count; }
 
 int b2_model_create(const b2_model_desc* desc, b2_model** out) {
@@ -1584,7 +1591,8 @@ static int copy_tokens_in(b2_kv* kv, const int32_t* tokens, int B, cudaStream_t 
 static int set_sampling(b2_kv* kv, const SampleState& v, bool force, cudaStream_t st) {
     const SampleState& c = kv->samp_host;
     if (!force && kv->samp_valid && c.do_sample == v.do_sample && c.temperature == v.temperature && c.top_p == v.top_p &&
-        c.top_k == v.top_k && c.seed == v.seed && c.tag == v.tag && c.per_row == v.per_row)
+        c.top_k == v.top_k && c.seed == v.seed && c.tag == v.tag && c.per_row == v.per_row && c.out_scores == v.out_scores &&
+        c.out_logits == v.out_logits && c.out_cap == v.out_cap)
         return 0;
     B2_TRY(sample_state_set(kv->sstate.as<SampleState>(), v, st));
     kv->samp_host = v;
@@ -1857,11 +1865,35 @@ int b2_op_beam_sample(const float* logits, const int32_t* row_of_beam, const flo
     return r;
 }
 
+int b2_op_beam_select_out(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
+                          const b2_beam_sampling* sampling, uint32_t step, int fan, float* out_scores, int32_t* out_tokens,
+                          int32_t* out_beams, float* row_scores, float* row_logits, void* stream) {
+    B2_CHECK_ARG(B >= 1 && nb >= 1 && nb <= 32 && K >= 1 && K <= 128, "b2_op_beam_select_out: B=%d nb=%d K=%d", B, nb, K);
+    B2_CHECK_ARG(fan >= 1 && fan <= 32 && (sampling == nullptr || fan == 1),
+                 "b2_op_beam_select_out: fan %d (1..32, and 1 with sampling)", fan);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    BeamRowsOut ro;
+    ro.scores = row_scores; ro.logits = row_logits; ro.fan = fan;
+    void* ws = nullptr;
+    B2_CUDA_CHECK(cudaMallocAsync(&ws, beam_sample_workspace_bytes(B, nb, K), st));  // >= beam_topk's
+    const int r = sampling != nullptr
+                      ? beam_sample(logits, row_of_beam, beam_scores, B, nb, V, K, beam_sample_params(sampling, step), ws, out_scores,
+                                    out_tokens, out_beams, st, ro)
+                      : beam_topk(logits, row_of_beam, beam_scores, B, nb, V, K, ws, out_scores, out_tokens, out_beams, st, ro);
+    B2_CUDA_CHECK(cudaFreeAsync(ws, st));
+    return r;
+}
+
 int b2_beam_step(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, void* stream) {
     return b2_beam_step_ex(m, kv, a, nullptr, 0u, stream);
 }
 
 int b2_beam_step_ex(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, const b2_beam_sampling* sampling, uint32_t step, void* stream) {
+    return b2_beam_step_out(m, kv, a, sampling, step, nullptr, nullptr, stream);
+}
+
+int b2_beam_step_out(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, const b2_beam_sampling* sampling, uint32_t step,
+                     float* row_scores, float* row_logits, void* stream) {
     B2_CHECK_ARG(m && kv && a && kv->m == m, "b2_beam_step: bad handle");
     B2_CHECK_ARG(m->finalized, "b2_beam_step: model not finalized");
     const int B = a->B, nb = a->nb, K = a->K, n = a->B * a->nb;
@@ -1914,11 +1946,13 @@ int b2_beam_step_ex(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, const b2
     int32_t* o_t = reinterpret_cast<int32_t*>(o_s + B * K);
     int32_t* o_b = o_t + B * K;
     const float* run_scores = reinterpret_cast<const float*>(rows + kv->max_batch);
+    BeamRowsOut ro;
+    ro.scores = row_scores; ro.logits = row_logits;
     if (sampling != nullptr)
         B2_TRY(beam_sample(m->logits.as<float>(), rows, run_scores, B, nb, m->d.vocab, K, beam_sample_params(sampling, step), kv->beam_ws.p,
-                           o_s, o_t, o_b, st));
+                           o_s, o_t, o_b, st, ro));
     else
-        B2_TRY(beam_topk(m->logits.as<float>(), rows, run_scores, B, nb, m->d.vocab, K, kv->beam_ws.p, o_s, o_t, o_b, st));
+        B2_TRY(beam_topk(m->logits.as<float>(), rows, run_scores, B, nb, m->d.vocab, K, kv->beam_ws.p, o_s, o_t, o_b, st, ro));
     B2_CUDA_CHECK(cudaMemcpyAsync(a->out_scores_host, o_s, (size_t)B * K * 4, cudaMemcpyDeviceToHost, st));
     B2_CUDA_CHECK(cudaMemcpyAsync(a->out_tokens_host, o_t, (size_t)B * K * 4, cudaMemcpyDeviceToHost, st));
     B2_CUDA_CHECK(cudaMemcpyAsync(a->out_beams_host, o_b, (size_t)B * K * 4, cudaMemcpyDeviceToHost, st));
@@ -1928,6 +1962,15 @@ int b2_beam_step_ex(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, const b2
 }
 
 // ---- streaming decode: the device runs ahead, the host reads tokens from mapped pinned memory ---------------------------
+int b2_stream_set_outputs(b2_kv* kv, float* scores, float* logits, int cap_steps) {
+    B2_CHECK_ARG(kv != nullptr, "b2_stream_set_outputs: null cache");
+    const bool any = scores != nullptr || logits != nullptr;
+    B2_CHECK_ARG(!any || cap_steps >= 1, "b2_stream_set_outputs: cap_steps %d must be >= 1", cap_steps);
+    std::lock_guard<std::mutex> lk(kv->m->mu);
+    kv->next_scores = scores; kv->next_logits = logits; kv->next_cap = any ? cap_steps : 0;
+    return 0;
+}
+
 int b2_stream_begin(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sp, void* stream) {
     return b2_stream_begin_ex(m, kv, logits, B, sp, nullptr, stream);
 }
@@ -1935,6 +1978,14 @@ int b2_stream_begin(b2_model* m, b2_kv* kv, const float* logits, int B, const b2
 int b2_stream_begin_ex(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sp, const b2_logits_proc* proc,
                        void* stream) {
     B2_CHECK_ARG(m && kv && logits && kv->m == m, "b2_stream_begin: bad handle");
+    // the rows armed by b2_stream_set_outputs belong to this call, whether or not it begins a generation
+    float *out_scores, *out_logits;
+    int out_cap;
+    {
+        std::lock_guard<std::mutex> lk(m->mu);
+        out_scores = kv->next_scores; out_logits = kv->next_logits; out_cap = kv->next_cap;
+        kv->next_scores = kv->next_logits = nullptr; kv->next_cap = 0;
+    }
     B2_CHECK_ARG(m->finalized, "b2_stream_begin: model not finalized");
     B2_CHECK_ARG(B >= 1 && B <= kv->max_batch, "b2_stream_begin: B=%d exceeds cache batch %d", B, kv->max_batch);
     SampleState v = {};
@@ -1948,6 +1999,7 @@ int b2_stream_begin_ex(b2_model* m, b2_kv* kv, const float* logits, int B, const
     std::lock_guard<std::mutex> lk(m->mu);
     DeviceGuard dg(m->device);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    v.out_scores = out_scores; v.out_logits = out_logits; v.out_cap = out_cap;
     for (int b = 0; b < B; ++b)
         B2_CHECK_ARG(kv->len_host[b] >= 1, "b2_stream_begin: sample %d has an empty cache (prefill first)", b);
     std::vector<ProcRow> pr(B);
@@ -1993,6 +2045,8 @@ int b2_stream_begin_lookup(b2_model* m, b2_kv* kv, const float* logits, int B, c
     std::lock_guard<std::mutex> lk_(m->mu);
     DeviceGuard dg(m->device);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    B2_CHECK_ARG(kv->next_scores == nullptr && kv->next_logits == nullptr,
+                 "b2_stream_begin_lookup: a prompt-lookup generation writes no score or logits rows (b2_stream_set_outputs)");
     // the last step writes rows up to len + (max_new_tokens - 1) + R - 1
     B2_CHECK_ARG(kv->len_host[0] >= 1 && (int64_t)kv->len_host[0] + lk->max_new_tokens + lk->num_tokens <= kv->max_seq,
                  "b2_stream_begin_lookup: cache length %d + max_new_tokens %d + num_tokens %d exceed max_seq %d", kv->len_host[0],
@@ -2124,6 +2178,8 @@ int b2_batch_begin(b2_model* m, b2_kv* kv, int B, void* stream) {
     std::lock_guard<std::mutex> lk(m->mu);
     DeviceGuard dg(m->device);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    B2_CHECK_ARG(kv->next_scores == nullptr && kv->next_logits == nullptr,
+                 "b2_batch_begin: a continuously batched cache writes no score or logits rows (b2_stream_set_outputs)");
     SampleState v = {};
     v.temperature = 1.f; v.top_p = 1.f; v.per_row = 1;
     kv->spec_R = 0;

@@ -167,6 +167,14 @@ sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleStat
     const bool proc_on = spec == nullptr && proc.rows != nullptr && proc.rows[b].on != 0 && active;
     int choice = 0;
     const float* row = logits + (size_t)b * V;
+    // output rows of token `pub` (generate(output_scores / output_logits)); a multi-row acceptance or an idle slot writes none
+    float* srow = nullptr;
+    if (select && spec == nullptr && !per_row && pub < st->out_cap) {
+        const size_t off = ((size_t)pub * B + b) * V;
+        if (st->out_scores != nullptr) srow = st->out_scores + off;
+        if (st->out_logits != nullptr)
+            for (int i = tid; i < V; i += SP_THREADS) st->out_logits[off + i] = row[i];
+    }
     if (select && (proc_on || processed_out != nullptr)) {
         // stage the row and run the processors in HF's order over it; selection below reads the staged row
         for (int i = tid; i < V; i += SP_THREADS) s_x[i] = row[i];
@@ -184,8 +192,14 @@ sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleStat
     } else if (!(flags & SP_SELECT)) {
         choice = tok[b];  // already chosen by the producer of `tok` (decode megakernel's fused argmax)
     } else if (!do_sample) {
+        if (srow != nullptr)  // greedy: the score row is the processed row the argmax reads
+            for (int i = tid; i < V; i += SP_THREADS) srow[i] = row[i];
         choice = block_argmax(row, V, tid, s_v, s_i, nullptr);
     } else {
+        // the score row is HF's x / T (IEEE division, TemperatureLogitsWarper); the draw keeps multiplying by 1 / T. Tokens the
+        // filters below remove become -inf in it where the draw's own rule removes them
+        if (srow != nullptr)
+            for (int i = tid; i < V; i += SP_THREADS) srow[i] = __fdiv_rn(row[i], temperature);
         const float inv_t = 1.0f / temperature;
         for (int i = tid; i < V; i += SP_THREADS) s_x[i] = row[i] * inv_t;  // in place when staged: each thread its own i
         __syncthreads();
@@ -196,7 +210,10 @@ sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleStat
                 V, (unsigned long long)k, tid, [&](int i) { return order_key(s_x[i]); }, [](int) { return 1ull; }, s_hist,
                 &s_prefix, &s_above);
             for (int i = tid; i < V; i += SP_THREADS)
-                if (order_key(s_x[i]) < kth) s_x[i] = -INFINITY;
+                if (order_key(s_x[i]) < kth) {
+                    s_x[i] = -INFINITY;
+                    if (srow != nullptr) srow[i] = -INFINITY;
+                }
             __syncthreads();
         }
         // ---- softmax numerators over the survivors: e_i = exp(x_i - max) (max itself always survives) ----
@@ -219,7 +236,10 @@ sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleStat
                 [&](int i) { return mass_of(s_x[i]); }, s_hist, &s_prefix, &s_above);
             for (int i = tid; i < V; i += SP_THREADS) {
                 const float x = s_x[i];
-                if (__float_as_uint(x > 0.f ? x : 0.f) < thr) s_x[i] = 0.f;
+                if (__float_as_uint(x > 0.f ? x : 0.f) < thr) {
+                    s_x[i] = 0.f;
+                    if (srow != nullptr) srow[i] = -INFINITY;
+                }
             }
             __syncthreads();
         }
@@ -372,6 +392,25 @@ proc_seed_kernel(ProcState proc, int row, ProcRow v, const int64_t* __restrict__
     if (tid == 0) proc.rows[row] = v;
 }
 
+// the output rows of a token the megakernel's fused argmax chose and published: grid (chunks, B), 256 threads
+constexpr int PR_THREADS = 256, PR_CHUNKS = 16;
+__global__ void __launch_bounds__(PR_THREADS)
+publish_rows_kernel(const float* __restrict__ logits, int V, int B, const SampleState* st) {
+    pdl_trigger();
+    pdl_wait();  // the logits and the publication counter are written by the megakernel before this launch
+    const int t = st->pub_counter - 1, b = blockIdx.y;
+    if (t < 0 || t >= st->out_cap) return;
+    const float* row = logits + (size_t)b * V;
+    const size_t off = ((size_t)t * B + b) * V;
+    float* s = st->out_scores;
+    float* l = st->out_logits;
+    for (int i = blockIdx.x * PR_THREADS + threadIdx.x; i < V; i += PR_CHUNKS * PR_THREADS) {
+        const float x = row[i];
+        if (s != nullptr) s[off + i] = x;
+        if (l != nullptr) l[off + i] = x;
+    }
+}
+
 __global__ void sample_state_set_kernel(SampleState* st, SampleState v) {
     if (threadIdx.x == 0) *st = v;
 }
@@ -388,6 +427,13 @@ size_t sample_smem_bytes(int V) { return (size_t)V * sizeof(float); }
 
 int sample_state_set(SampleState* st_dev, const SampleState& v, cudaStream_t stream) {
     sample_state_set_kernel<<<1, 32, 0, stream>>>(st_dev, v);
+    B2_LAUNCH_CHECK();
+    return 0;
+}
+
+int publish_rows(const float* logits, int V, int B, const SampleState* st_dev, cudaStream_t stream) {
+    B2_CHECK_ARG(logits != nullptr && st_dev != nullptr && B >= 1 && V >= 1, "publish_rows: bad argument");
+    B2_CUDA_CHECK(launch_pdl(publish_rows_kernel, dim3(PR_CHUNKS, B), dim3(PR_THREADS), 0, stream, logits, V, B, st_dev));
     B2_LAUNCH_CHECK();
     return 0;
 }

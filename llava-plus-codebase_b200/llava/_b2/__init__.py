@@ -174,6 +174,7 @@ SIGNATURES = {
     "b2_stream_begin_ex": (_i32, [_vp, _vp, _vp, _i32, _c.POINTER(Sampling), _c.POINTER(LogitsProc), _vp]),
     "b2_stream_enqueue": (_i32, [_vp, _vp, _i32, _vp]),
     "b2_stream_wait": (_i32, [_vp, _i32, _c.POINTER(_c.c_int32), _i32]),
+    "b2_stream_set_outputs": (_i32, [_vp, _vp, _vp, _i32]),
     "b2_stream_begin_lookup": (_i32, [_vp, _vp, _vp, _i32, _c.POINTER(Sampling), _c.POINTER(PromptLookup), _vp]),
     "b2_stream_lookup_stats": (_i32, [_vp, _c.POINTER(_c.c_int32), _c.POINTER(_c.c_int32), _c.POINTER(_c.c_int32)]),
     "b2_decode_rows": (_i32, [_vp, _vp, _i32, _vp, _i32, _vp, _vp]),
@@ -194,6 +195,9 @@ SIGNATURES = {
     "b2_beam_step": (_i32, [_vp, _vp, _c.POINTER(BeamStepArgs), _vp]),
     "b2_op_beam_sample": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _c.POINTER(BeamSampling), _c.c_uint32, _vp, _vp, _vp, _vp]),
     "b2_beam_step_ex": (_i32, [_vp, _vp, _c.POINTER(BeamStepArgs), _c.POINTER(BeamSampling), _c.c_uint32, _vp]),
+    "b2_op_beam_select_out": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _c.POINTER(BeamSampling), _c.c_uint32, _i32, _vp, _vp,
+                                     _vp, _vp, _vp, _vp]),
+    "b2_beam_step_out": (_i32, [_vp, _vp, _c.POINTER(BeamStepArgs), _c.POINTER(BeamSampling), _c.c_uint32, _vp, _vp, _vp]),
     "b2_op_gemm": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "b2_op_gemv": (_i32, [_vp, _i64, _vp, _i32, _vp, _f32, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "b2_op_quantize_nf4": (_i32, [_vp, _i32, _i32, _vp, _vp, _vp]),
@@ -511,14 +515,25 @@ class Engine:
         return out
 
     # -- streaming decode (device runs ahead, host reads tokens from mapped pinned memory) ---------------
-    def stream_begin(self, kv, logits, sampling=None, procs=None):
+    def stream_begin(self, kv, logits, sampling=None, procs=None, out_scores=None, out_logits=None):
         """Token 0 is chosen from the prefill logits [B, vocab] on the device and published as ring index 0. `procs`: one
-        LogitsProc (or None) per row; rows with processors keep their history on the device for the whole generation."""
+        LogitsProc (or None) per row; rows with processors keep their history on the device for the whole generation.
+        `out_scores` / `out_logits` (device fp32 [steps, B, vocab], or None): the step that publishes token t writes its score
+        row (what selection read: processed, and when sampling divided by T and filtered) and its raw logits row to index t
+        (b2_stream_set_outputs). Keep them alive until the generation's steps have run."""
         logits = logits.contiguous()
         sp = sampling if sampling is not None else make_sampling()
         B = int(logits.shape[0])
         arr = _proc_array(procs, B)
+        cap = 0
+        for o in (out_scores, out_logits):
+            if o is not None:
+                if o.dtype != torch.float32 or o.dim() != 3 or tuple(o.shape[1:]) != (B, self.vocab) or not o.is_contiguous():
+                    raise ValueError(f"output rows must be contiguous fp32 [steps, {B}, {self.vocab}], got {tuple(o.shape)}")
+                cap = int(o.shape[0]) if cap == 0 else min(cap, int(o.shape[0]))
         with torch.cuda.device(self.index):
+            # always armed (NULLs included): a begin never inherits buffers a failed call left behind
+            check(self.lib.b2_stream_set_outputs(kv.handle, ptr(out_scores), ptr(out_logits), cap), "b2_stream_set_outputs")
             if arr is None:
                 check(self.lib.b2_stream_begin(self.handle, kv.handle, ptr(logits), B, ctypes.byref(sp), stream_ptr()),
                       "b2_stream_begin")
@@ -634,11 +649,34 @@ class Engine:
                                              int(step), ptr(out_s), ptr(out_t), ptr(out_b), stream_ptr()), "b2_op_beam_sample")
         return out_s, out_t, out_b
 
-    def beam_step(self, kv, copies, row_begin, tokens, slot_of_beam, beam_scores, nb, K, sampling=None, step=0):
+    def beam_select_out(self, logits, beam_scores, nb, K, row_scores, row_logits, sampling=None, step=0, row_of_beam=None, fan=1):
+        """beam_topk (or beam_sample with `sampling`) that also writes each beam row's score row (log_softmax, warped under
+        sampling) and raw logits row to row_scores / row_logits (device fp32 [B*nb*fan, V] or None), `fan` copies per beam
+        row (b2_op_beam_select_out)."""
+        V = logits.shape[-1]
+        scores = beam_scores.to(device=self.device, dtype=torch.float32).contiguous()
+        B = scores.numel() // nb
+        rows = None if row_of_beam is None else torch.as_tensor(row_of_beam, dtype=torch.int32).to(self.device).contiguous()
+        for o in (row_scores, row_logits):
+            if o is not None and (o.dtype != torch.float32 or o.numel() != B * nb * fan * V or not o.is_contiguous()):
+                raise ValueError(f"output rows must be contiguous fp32 [{B * nb * fan}, {V}]")
+        out_s = torch.empty(B, K, dtype=torch.float32, device=self.device)
+        out_t = torch.empty(B, K, dtype=torch.int32, device=self.device)
+        out_b = torch.empty(B, K, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.index):
+            check(self.lib.b2_op_beam_select_out(ptr(logits), ptr(rows), ptr(scores), B, int(nb), V, int(K),
+                                                 None if sampling is None else ctypes.byref(sampling), int(step), int(fan), ptr(out_s),
+                                                 ptr(out_t), ptr(out_b), ptr(row_scores), ptr(row_logits), stream_ptr()),
+                  "b2_op_beam_select_out")
+        return out_s, out_t, out_b
+
+    def beam_step(self, kv, copies, row_begin, tokens, slot_of_beam, beam_scores, nb, K, sampling=None, step=0, row_scores=None,
+                  row_logits=None):
         """One step of the running beams (b2_beam_step, or b2_beam_step_ex with a BeamSampling): `copies` = [(src, dst)] applied
         first, tokens[i] fed to slot slot_of_beam[i], one decode step at batch len(tokens), candidates of every sample selected
         (or, with `sampling`, drawn as draw `step`) on the device. Returns CPU tensors (scores fp32, tokens int64, beams int64),
-        each [B, K], best (or first drawn) first."""
+        each [B, K], best (or first drawn) first. `row_scores` / `row_logits` (device fp32 [len(tokens), V] or None) receive the
+        step's score rows and raw logits rows in beam order (b2_beam_step_out)."""
         n = len(tokens)
         B = n // nb
         i32 = lambda xs: (_c.c_int32 * max(len(xs), 1))(*[int(x) for x in xs])
@@ -652,7 +690,14 @@ class Engine:
                          _c.cast(slots, _vp), _c.cast(scores, _vp), _vp(out_s.data_ptr()), _vp(out_t.data_ptr()),
                          _vp(out_b.data_ptr()))
         with torch.cuda.device(self.index):
-            if sampling is None:
+            if row_scores is not None or row_logits is not None:
+                for o in (row_scores, row_logits):
+                    if o is not None and (o.dtype != torch.float32 or o.numel() != n * self.vocab or not o.is_contiguous()):
+                        raise ValueError(f"output rows must be contiguous fp32 [{n}, {self.vocab}]")
+                check(self.lib.b2_beam_step_out(self.handle, kv.handle, ctypes.byref(a),
+                                                None if sampling is None else ctypes.byref(sampling), int(step), ptr(row_scores),
+                                                ptr(row_logits), stream_ptr()), "b2_beam_step_out")
+            elif sampling is None:
                 check(self.lib.b2_beam_step(self.handle, kv.handle, ctypes.byref(a), stream_ptr()), "b2_beam_step")
             else:
                 check(self.lib.b2_beam_step_ex(self.handle, kv.handle, ctypes.byref(a), ctypes.byref(sampling), int(step),

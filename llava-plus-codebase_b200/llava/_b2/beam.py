@@ -4,7 +4,9 @@
 `_get_running_beams_for_next_iteration`, `_update_finished_beams`, `_check_early_stop_heuristic`,
 `_beam_search_has_unfinished_sequences`) over the K = max(2, 1 + n_eos) * num_beams candidates per sample that the device
 selects each step (b2_op_beam_topk / b2_beam_step): running beams, finished hypotheses with their length penalty, the early-stop
-heuristic, termination and the output tensor. The arithmetic on scores is HF's, in fp32 on the CPU, in HF's order.
+heuristic, termination and the output tensor. The arithmetic on scores is HF's, in fp32 on the CPU, in HF's order. Beside the
+running and finished sequences it carries HF's beam-index tensors (the flat running beam b * num_beams + j each generated token
+came from), gathered the same way, for generate(return_dict_in_generate=True)'s `beam_indices`.
 
 `SlotPlanner` keeps the map from running beam to KV-cache slot and turns each step's parent vector into a list of slot copies:
 a parent's first child stays in the parent's slot (it only appends a row); every further child takes the slot of a parent that
@@ -66,6 +68,9 @@ class BeamSearch:
         self.top_mask = torch.cat([torch.ones(nb, dtype=torch.bool), torch.zeros(self.K - nb, dtype=torch.bool)])
         self.cur_len = self.Lt
         self.parents = torch.zeros(B, nb, dtype=torch.int64)          # running beam j came from beam parents[b, j]
+        # HF's running / finished beam indices: int32, -1 where nothing was generated
+        self.running_beam_indices = torch.full((B, nb, self.max_length - self.Lt), -1, dtype=torch.int32)
+        self.beam_indices = self.running_beam_indices.clone()
         self.done = False
 
     @staticmethod
@@ -83,6 +88,8 @@ class BeamSearch:
         topk_beams = topk_beams.to("cpu", torch.int64).reshape(B, K)
         cand = self._gather(self.running, topk_beams)
         cand[:, :, cur] = topk_tokens
+        cand_bi = self._gather(self.running_beam_indices, topk_beams)
+        cand_bi[:, :, cur - self.Lt] = (topk_beams + torch.arange(B).view(-1, 1) * nb).to(torch.int32)
         hits = stopping_hits(cand[:, :, :cur + 1].reshape(B * K, cur + 1), self.criteria, self.max_length,
                              self.eos_ids).reshape(B, K)
 
@@ -91,6 +98,7 @@ class BeamSearch:
         nxt = torch.topk(run_scores, k=nb)[1]
         self.running = self._gather(cand, nxt)
         self.running_scores = self._gather(run_scores, nxt)
+        self.running_beam_indices = self._gather(cand_bi, nxt)
         self.parents = self._gather(topk_beams, nxt)
 
         # finished hypotheses: candidates among the first num_beams that hit a criterion, length-normalised
@@ -104,11 +112,13 @@ class BeamSearch:
         m_scores = torch.cat((self.beam_scores, s), dim=1)
         m_len = torch.cat((self.gen_len, torch.full((B, K), cur + 1 - self.Lt, dtype=torch.int64)), dim=1)
         m_fin = torch.cat((self.is_sent_finished, did), dim=1)
+        m_bi = torch.cat((self.beam_indices, cand_bi), dim=1)
         keep = torch.topk(m_scores, k=nb)[1]
         self.sequences = self._gather(m_seq, keep)
         self.beam_scores = self._gather(m_scores, keep)
         self.gen_len = self._gather(m_len, keep)
         self.is_sent_finished = self._gather(m_fin, keep)
+        self.beam_indices = self._gather(m_bi, keep)
 
         self.cur_len = cur = cur + 1
         if self.early_stopping == "never" and self.length_penalty > 0.0:
@@ -133,6 +143,14 @@ class BeamSearch:
         seq = self.sequences[:, :r].reshape(self.B * r, -1)
         n = int(self.gen_len[:, :r].max())
         return seq[:, :self.Lt + n].clone(), self.beam_scores[:, :r].reshape(-1).clone()
+
+    def output_beam_indices(self):
+        """HF's `beam_indices` of the returned sequences: int32 [B * num_return_sequences, longest returned continuation], the
+        flat running beam each generated token came from, -1 past a sequence's end."""
+        r = self.num_return_sequences
+        bi = self.beam_indices[:, :r].reshape(self.B * r, -1)
+        n = int(((bi + 1) != 0).sum(dim=1).max())
+        return bi[:, :n].clone()
 
 
 class SlotPlanner:

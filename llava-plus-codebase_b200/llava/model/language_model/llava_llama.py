@@ -491,7 +491,7 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
     def generate(self, inputs=None, images=None, do_sample=False, temperature=1.0, top_p=None, top_k=None,
                  num_beams=1, max_new_tokens=None, max_length=None, use_cache=True, streamer=None,
                  stopping_criteria=None, eos_token_id=None, pad_token_id=None, attention_mask=None,
-                 input_ids=None, output_scores=False, return_dict_in_generate=False, **kwargs):
+                 input_ids=None, output_scores=False, return_dict_in_generate=False, output_logits=False, **kwargs):
         """Own decoding loop with the side-protocols the reference's callers rely on (SURVEY §8b): prompt ids (with
         IMAGE_TOKEN_INDEX) echoed in the result, `streamer.put/end`, `stopping_criteria` called as
         crit(ids_so_far, scores) -> bool | bool tensor, eos stop, temperature / top-k / top-p sampling.
@@ -499,11 +499,24 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         Every variant runs the same device-resident loop: token feedback, argmax or the sampling draw are kernels, each
         step publishes its token into pinned host memory, and this thread (usually a worker `Thread`,
         llava/serve/model_worker.py:174-185) reads token t — streamer, eos, stopping criteria — while the device is
-        already `config.b2_run_ahead` (default 8) steps further. Steps queued beyond the stop point are discarded."""
+        already `config.b2_run_ahead` (default 8) steps further. Steps queued beyond the stop point are discarded.
+
+        With return_dict_in_generate=True the result is transformers' GenerateDecoderOnlyOutput (GenerateBeamDecoderOnlyOutput
+        with num_beams > 1): `scores` (output_scores) and `logits` (output_logits) are tuples of one fp32 tensor per generated
+        step on the model's device, [B, V] ([B * num_beams, V] for beams, in the running-beam order). A score row is what HF
+        hands to selection: the logits after the processors, and when sampling x / T with the tokens top-k / top-p remove at
+        -inf; under beam search log_softmax(logits), warped under beam sampling. The decode kernels write the rows while the
+        device runs ahead, so they cost no synchronisation per token. A row of a batch that has finished keeps decoding its own
+        tokens (the result shows pad there), so its scores and logits after its eos are not the ones HF, which feeds it pad
+        ids, would give; every position up to and including its eos is. `past_key_values`, `attentions` and `hidden_states`
+        are None. Stopping criteria still receive scores=None: handing them the live device rows would need a synchronisation
+        per token. Without return_dict_in_generate the id tensor is returned and output_scores / output_logits are ignored,
+        as in HF."""
         if inputs is None:
             inputs = input_ids
         if inputs is None:
             raise ValueError("generate() needs input ids")
+        want = _output_arguments(return_dict_in_generate, output_scores, output_logits, kwargs)
         proc_args = self._logits_processor_arguments(kwargs)
         beam_args = {}
         if num_beams != 1:
@@ -512,12 +525,15 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                                           "min_length) together with num_beams > 1 are not implemented on the H100 path")
             if self._beam_search_cap() < 2:
                 raise NotImplementedError("beam search is not used on the LLaVA path (num_beams=1 everywhere)")
-            beam_args = self._beam_arguments(num_beams, do_sample, temperature, top_p, top_k, streamer, output_scores,
-                                             return_dict_in_generate, kwargs)
-        if return_dict_in_generate or output_scores:
-            raise NotImplementedError("generate() returns the id tensor only")
+            beam_args = self._beam_arguments(num_beams, do_sample, temperature, top_p, top_k, streamer, kwargs)
         prompt = inputs if inputs.dim() == 2 else inputs.unsqueeze(0)
         lookup_args = self._prompt_lookup_arguments(kwargs, prompt.shape[0], num_beams, bool(proc_args))
+        if want and (want["scores"] or want["logits"]):
+            what = "output_scores / output_logits with return_dict_in_generate"
+            if lookup_args:
+                raise NotImplementedError(f"{what} together with the prompt-lookup path (b2_prompt_lookup) is not implemented")
+            if prompt.shape[0] == 1 and num_beams == 1 and int(getattr(self.config, "b2_continuous_batching", 0) or 0) >= 2:
+                raise NotImplementedError(f"{what} together with the continuous batcher (b2_continuous_batching) is not implemented")
         for k, v in kwargs.items():
             if k in self._IGNORED_GENERATION_ARGS:
                 continue
@@ -539,7 +555,7 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             eos_list = (list(eos_token_id) if isinstance(eos_token_id, (list, tuple))
                         else (None if eos_token_id is None else [eos_token_id]))
             return self._beam_generate(engine, prompt, images, attention_mask, num_beams, max_new_tokens, eos_list, pad_token_id,
-                                       stopping_criteria, **beam_args)
+                                       stopping_criteria, want=want, **beam_args)
         greedy = (not do_sample) or (temperature is not None and temperature <= 1e-5)
         if greedy:
             sampling = make_sampling()
@@ -593,8 +609,12 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 req.cancel()
             if streamer is not None:
                 streamer.end()
-            return torch.cat([prompt, new_tokens.to(device=prompt.device, dtype=prompt.dtype)], dim=1)
+            out = torch.cat([prompt, new_tokens.to(device=prompt.device, dtype=prompt.dtype)], dim=1)
+            return out if not want else _decoder_output(out, None, None)
 
+        # score / logits rows of every step the generation may take, written by the device (b2_stream_set_outputs)
+        rows = {k: (torch.empty(max_new_tokens, B, engine.vocab, dtype=torch.float32, device=engine.device) if want and want[k] else None)
+                for k in ("scores", "logits")}
         # conversation prefix reuse (opt-in, batch 1): the part of the prompt a released cache already holds is not prefilled again
         plan = None
         if B == 1 and self._prefix_cache_on() and (attention_mask is None or bool(attention_mask.bool().all())):
@@ -618,13 +638,14 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 if lk is not None:
                     engine.stream_begin_lookup(kv, logits, sampling, lk)
                 else:
-                    engine.stream_begin(kv, logits, sampling, procs)
+                    engine.stream_begin(kv, logits, sampling, procs, rows["scores"], rows["logits"])
                 engine.stream_wait(kv, 0, B)          # first sync of this call: every input check has run by now
                 if prof: prof.mark("prefill + first token")
                 return speculative
 
             if plan is not None:
-                began_lookup[0] = self._prefill_reusing(engine, kv, plan, reuse, released_ev, sampling, max_new_tokens, procs, lookup)
+                began_lookup[0] = self._prefill_reusing(engine, kv, plan, reuse, released_ev, sampling, max_new_tokens, procs, lookup,
+                                                        rows)
                 speculative = False
             else:
                 speculative = prefill(False)
@@ -655,7 +676,17 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             streamer.end()
         out = torch.cat([prompt, new_tokens.to(device=prompt.device, dtype=prompt.dtype)], dim=1)
         if prof: prof.mark("ids to caller"); prof.report()
-        return out
+        if not want:
+            return out
+        n = new_tokens.shape[1]
+        return _decoder_output(out, _trim_steps(rows.pop("scores"), n), _trim_steps(rows.pop("logits"), n))
+
+    def compute_transition_scores(self, sequences, scores, beam_indices=None, normalize_logits=False):
+        """transformers' GenerationMixin.compute_transition_scores: the score of each generated token from generate()'s
+        `scores` (and `beam_indices` after beam search), [batch * num_return_sequences, generated length]."""
+        from transformers.generation.utils import GenerationMixin
+
+        return GenerationMixin.compute_transition_scores(self, sequences, scores, beam_indices, normalize_logits)
 
     def _prompt_embeds(self, engine, prompt, attention_mask, images, force_host):
         """Spliced prompt rows of generate(): (embeds [B, S, hidden], valid rows per sample, whether the device splice was
@@ -779,8 +810,7 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         v = getattr(self.config, "b2_beam_sample", None)
         return bool(v) if v is not None else os.environ.get("B2_BEAM_SAMPLE") == "1"
 
-    def _beam_arguments(self, num_beams, do_sample, temperature, top_p, top_k, streamer, output_scores, return_dict_in_generate,
-                        kwargs):
+    def _beam_arguments(self, num_beams, do_sample, temperature, top_p, top_k, streamer, kwargs):
         """Checks what generate(num_beams > 1) does not implement and takes the beam-only arguments out of `kwargs`. With
         do_sample (and a temperature above 1e-5, below which it is beam search) the result carries `sampling`: the warpers of
         beam sampling, HF GenerationConfig's defaults top_k = 50 and top_p = 1.0 filled in."""
@@ -794,8 +824,6 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             raise NotImplementedError("group beam search (num_beam_groups / diversity_penalty) is not implemented on the H100 path")
         if kwargs.get("constraints") is not None:
             raise NotImplementedError("constrained beam search (constraints) is not implemented on the H100 path")
-        if output_scores or return_dict_in_generate:
-            raise NotImplementedError("beam search returns the id tensor only (output_scores / return_dict_in_generate)")
         if streamer is not None:
             raise ValueError("`streamer` cannot be used with beam search (num_beams > 1)")
         sampling = None
@@ -813,7 +841,7 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                     num_return_sequences=1 if nrs is None else int(nrs), sampling=sampling)
 
     def _beam_generate(self, engine, prompt, images, attention_mask, num_beams, max_new_tokens, eos_ids, pad_token_id,
-                       stopping_criteria, length_penalty, early_stopping, num_return_sequences, sampling=None):
+                       stopping_criteria, length_penalty, early_stopping, num_return_sequences, sampling=None, want=None):
         """Beam search (llava/_b2/beam.py): sample b is prefilled once into slot b of a pool cache; its candidates from the
         prefill logits fork the prompt into nb slots; then every b2_beam_step applies the step's slot copies, decodes the
         B * nb running beams in one batch and returns the K best candidates per sample for the host bookkeeping.
@@ -821,7 +849,10 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         With `sampling` (beam sampling) the device draws the K candidates of step t with b2_op_beam_sample / b2_beam_step_ex at
         draw index t, seeded from torch's CPU generator. The first draw reads all nb beam rows of a sample, each mapped to its
         prefill row, with running scores [0, -1e9, ...] as HF's first step does: the -1e9 rows matter to which candidates fill
-        the list when fewer than K have positive probability."""
+        the list when fewer than K have positive probability.
+
+        `want` (generate()'s _output_arguments): the device also writes each step's score and raw logits rows, [B * nb, V] in
+        running-beam order, and the result is a GenerateBeamDecoderOnlyOutput."""
         from ..._b2 import beam as _beam
 
         B = prompt.shape[0]
@@ -837,6 +868,9 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             seed = int(torch.randint(0, 2**62, (1,), dtype=torch.int64).item())
             bs = make_beam_sampling(sampling["temperature"], sampling["top_k"], sampling["top_p"], min_keep, seed)
         self._check_limits(engine, B * nb, 1)
+        rows = {k: (torch.empty(max_new_tokens, B * nb, engine.vocab, dtype=torch.float32, device=engine.device)
+                    if want and want[k] else None) for k in ("scores", "logits")}
+        at = lambda k, t: None if rows[k] is None else rows[k][t]  # noqa: E731  (step t's [B * nb, V] rows)
         kv = self._pool.acquire()  # exclusive for this call; never recorded for prefix reuse
         try:
             def first_candidates(force_host):
@@ -844,7 +878,17 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 self._check_limits(engine, B * nb, max(lens) + max_new_tokens)
                 kv.reset()
                 logits = engine.prefill(kv, embeds, lens, LOGITS_LAST)
-                if bs is None:
+                if want:  # the same selection, also writing step 0's rows (the one prefill row of a sample fills its nb rows)
+                    if bs is None:
+                        cand = engine.beam_select_out(logits, torch.zeros(B), 1, search.K, at("scores", 0), at("logits", 0), fan=nb)
+                    else:
+                        cand = engine.beam_select_out(logits, search.running_scores.reshape(-1), nb, search.K, at("scores", 0),
+                                                      at("logits", 0), sampling=bs, step=0,
+                                                      row_of_beam=[b for b in range(B) for _ in range(nb)])
+                    cand = [t.cpu() for t in cand]
+                    if bs is not None:
+                        cand[2].zero_()
+                elif bs is None:
                     cand = [t.cpu() for t in engine.beam_topk(logits, torch.zeros(B), 1, search.K)]  # synchronises
                 else:
                     cand = [t.cpu() for t in engine.beam_sample(logits, search.running_scores.reshape(-1), nb, search.K, bs, 0,
@@ -866,12 +910,23 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 step += 1
                 copies = planner.plan(search.parents)
                 cand = engine.beam_step(kv, copies, row_begin, search.next_tokens().tolist(), planner.flat(),
-                                        search.running_scores.reshape(-1).tolist(), nb, search.K, sampling=bs, step=step)
+                                        search.running_scores.reshape(-1).tolist(), nb, search.K, sampling=bs, step=step,
+                                        **({"row_scores": at("scores", step), "row_logits": at("logits", step)} if want else {}))
                 row_begin = min(lens)
             engine.check_async_error()
         finally:
             self._pool.release(kv)
-        return search.output()[0].to(device=prompt.device, dtype=prompt.dtype)
+        seq, seq_scores = search.output()
+        seq = seq.to(device=prompt.device, dtype=prompt.dtype)
+        if not want:
+            return seq
+        from transformers.generation.utils import GenerateBeamDecoderOnlyOutput
+
+        n = search.cur_len - search.Lt  # steps taken: b2_beam_step synchronised on every one
+        return GenerateBeamDecoderOnlyOutput(
+            sequences=seq, sequences_scores=seq_scores.to(engine.device) if want["scores"] else None,
+            scores=_trim_steps(rows.pop("scores"), n), logits=_trim_steps(rows.pop("logits"), n),
+            beam_indices=search.output_beam_indices().to(engine.device), attentions=None, hidden_states=None, past_key_values=None)
 
     def _prefix_cache_on(self):
         """config.b2_prefix_cache or B2_PREFIX_CACHE=1 (off by default: logits of reused answer rows, which the decode kernels
@@ -905,11 +960,12 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             return None
         return {"items": items, "slots": slots, "images": images}
 
-    def _prefill_reusing(self, engine, kv, plan, m, released_ev, sampling, max_new_tokens, procs=None, lookup=None):
+    def _prefill_reusing(self, engine, kv, plan, m, released_ev, sampling, max_new_tokens, procs=None, lookup=None, out_rows=None):
         """Prefill of a planned prompt that keeps the first m spliced rows of `kv`: image slots wholly inside them are not
         encoded, rows [m, L) are spliced on the host-index path and prefilled at position m (b2_prefill_at). m == 0 is an
         ordinary prefill from position 0. Chooses and publishes token 0 like generate()'s own prefill. Returns whether the
-        generation decodes with prompt lookup (`lookup`: generate()'s lookup(rows) or None)."""
+        generation decodes with prompt lookup (`lookup`: generate()'s lookup(rows) or None). `out_rows`: generate()'s score / logits
+        buffers ({"scores", "logits"}, entries may be None)."""
         P = engine.num_patches
         items, slots = plan["items"], plan["slots"]
         rows = [_prefix.item_rows(x, P) for x in slots]
@@ -946,7 +1002,8 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         if lk is not None:
             engine.stream_begin_lookup(kv, logits, sampling, lk)
         else:
-            engine.stream_begin(kv, logits, sampling, procs)
+            out_rows = out_rows or {}
+            engine.stream_begin(kv, logits, sampling, procs, out_rows.get("scores"), out_rows.get("logits"))
         engine.stream_wait(kv, 0, 1)
         return lk is not None
 
@@ -1017,6 +1074,36 @@ def _check_weight_format(config):
     if fmt == "nf4" and (getattr(config, "b2_fp8_decode", False) or os.environ.get("B2_FP8_DECODE") == "1"):
         raise ValueError("b2_weight_format='nf4' (load_4bit) cannot be combined with b2_fp8_decode (e4m3 decode weights)")
     return fmt
+
+
+def _output_arguments(return_dict_in_generate, output_scores, output_logits, kwargs):
+    """{"scores", "logits"}: which per-step rows a generate(return_dict_in_generate=True) call returns, or None when generate()
+    returns the id tensor (output_scores / output_logits are then ignored, as HF ignores them)."""
+    if not return_dict_in_generate:
+        return None
+    for k in ("output_attentions", "output_hidden_states"):
+        if kwargs.get(k):
+            raise NotImplementedError(f"{k}=True with return_dict_in_generate: attention maps / hidden states are never "
+                                      "materialised on the fused path")
+    return {"scores": bool(output_scores), "logits": bool(output_logits)}
+
+
+def _trim_steps(buf, n):
+    """generate()'s rows [max_new_tokens, rows, V] -> a tuple of the first n steps' [rows, V] tensors. The decode steps were
+    ordered before later work on the caller's current stream when they were queued, so reading there is safe; a buffer with
+    an unused tail is copied, so the tail is not kept alive by the returned views."""
+    if buf is None:
+        return None
+    if n < buf.shape[0]:
+        buf = buf[:n].clone()
+    return tuple(buf.unbind(0))
+
+
+def _decoder_output(sequences, scores, logits):
+    from transformers.generation.utils import GenerateDecoderOnlyOutput
+
+    return GenerateDecoderOnlyOutput(sequences=sequences, scores=scores, logits=logits, attentions=None, hidden_states=None,
+                                     past_key_values=None)
 
 
 # verify steps a prompt-lookup generation keeps queued in front of the host: two keep the device busy while the host handles a
