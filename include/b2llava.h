@@ -228,7 +228,7 @@ int b2_stream_begin(b2_model* m, b2_kv* kv, const float* logits, int B, const b2
  * prefill logits over the prompt history; every later step of the generation processes against the history kept on the
  * device (prompt, then each chosen token). The cache's processing state is allocated by the first call that turns a processor
  * on (b2_kv_bytes does not count it). b2_stream_begin, b2_batch_begin, b2_decode_step, b2_decode_greedy and b2_beam_step turn
- * every row's processors off. -1 for repetition_penalty <= 0, a negative n-gram size, n_eos outside [0, 8] or a prompt longer
+ * every row's processors off, and disarm the processing of a beam search (b2_beam_begin_proc). -1 for repetition_penalty <= 0, a negative n-gram size, n_eos outside [0, 8] or a prompt longer
  * than the cache's max_seq. */
 int b2_stream_begin_ex(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sampling, const b2_logits_proc* proc,
                        void* stream);
@@ -370,6 +370,32 @@ int b2_op_beam_select_out(const float* logits, const int32_t* row_of_beam, const
                           int32_t* out_beams, float* row_scores, float* row_logits, void* stream);
 int b2_beam_step_out(b2_model* m, b2_kv* kv, const b2_beam_step_args* args, const b2_beam_sampling* sampling, uint32_t step,
                      float* row_scores, float* row_logits, void* stream);
+
+/* Logits processors in beam search (generate(num_beams > 1, repetition_penalty / no_repeat_ngram_size / min_new_tokens /
+ * min_length): HF 5.5 _beam_search runs them over each running beam's log_softmax row against that beam's own sequence, before the
+ * running score is added and, under beam sampling, before temperature / top-k / top-p). The processors of b2_logits_proc act on
+ * the fp32 log-probabilities ((x - max) - lse): a penalised history id's score is multiplied by p when negative; a log-prob of
+ * exactly 0 stays 0. The score rows written (row_scores) are the processed rows (warped under sampling).
+ *   b2_op_beam_select_proc  b2_op_beam_select_out over `rows` logits rows, where logits row r is processed against the history
+ *                           proc[r].prompt_ids (proc: [rows] structs, NULL = every row off; row_of_beam NULL needs rows == B*nb).
+ *                           Every beam row that reads logits row r (fan, row_of_beam) sees the same processed row. With every
+ *                           processor off, candidates and rows are those of b2_op_beam_select_out. Synchronises the stream.
+ *   b2_beam_begin_proc      arms the processing of a beam search on the cache: slot b < B gets proc[b] (NULL entry or NULL
+ *                           array = off) with its history seeded from proc[b]'s prompt ids; every other slot is off. Call it after
+ *                           the prompts are prefilled into slots 0..B-1, before the first b2_beam_step_proc.
+ *   b2_beam_step_proc       b2_beam_step_out with the armed processing: a copy moves the source slot's history (ids, presence
+ *                           bitmap and counters) with its K/V rows; then tokens_host[i] joins the history of slot
+ *                           slot_of_beam_host[i], and beam i's log_softmax row is processed against that history before selection.
+ *                           The decode step inside neither processes nor appends. One more kernel launch than b2_beam_step_out
+ *                           (the tokens to the device), plus one per 64 copies when the step copies slots.
+ * -1 (nothing queued) for the checks of b2_stream_begin_ex on a processor, and from b2_beam_step_proc on a cache where the
+ * processing is not armed. The calls that turn every row's processors off (see b2_stream_begin_ex) disarm it. */
+int b2_op_beam_select_proc(const float* logits, int rows, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V,
+                           int K, const b2_beam_sampling* sampling, uint32_t step, int fan, const b2_logits_proc* proc, float* out_scores,
+                           int32_t* out_tokens, int32_t* out_beams, float* row_scores, float* row_logits, void* stream);
+int b2_beam_begin_proc(b2_model* m, b2_kv* kv, int B, const b2_logits_proc* proc, void* stream);
+int b2_beam_step_proc(b2_model* m, b2_kv* kv, const b2_beam_step_args* args, const b2_beam_sampling* sampling, uint32_t step,
+                      float* row_scores, float* row_logits, void* stream);
 
 /* ---- single-kernel entry points (unit-level parity tests; same kernels the hot path launches) ----------- */
 int b2_op_gemm(const void* A, int lda, const void* W, int ldw, const void* bias, const void* residual, int ld_res,

@@ -13,6 +13,10 @@
 //     The K largest keys in order are HF's torch.multinomial(softmax(acc), K) draw order (multinomial without replacement is
 //     top-K of p / Exp(1) there). Warped-away tokens (-inf) rank below every finite key by index, NaN logits below those. The
 //     merge carries each candidate's unperturbed score acc beside its key.
+//   * with logits processors (BeamProc, b2_beam_step_proc / b2_op_beam_select_proc): both row kernels turn the staged row into
+//     log-probabilities, run HF's processors over them against the history of the row's cache slot (logits_proc.cuh's
+//     process_row, after appending the token the step fed to that slot), and rank on processed + running score; under beam
+//     sampling the warpers follow the processors. Instantiated separately (PROC = true), so the unprocessed kernels are unchanged.
 //   * kv_copy_slots: cache slot dst := rows [row_begin, end) of slot src for every layer, head, K and V (and the fp32 scale
 //     rows of an e4m3 cache); one (layer, head, K|V) slab of one slot is contiguous, so each CTA streams 64 rows with
 //     16-byte vectors. The caller guarantees that no dst is also a src (b2_kv_copy_slots checks it), so pairs are independent.
@@ -21,6 +25,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "logits_proc.cuh"
 #include "select.cuh"
 
 namespace b2 {
@@ -125,9 +130,27 @@ __device__ __forceinline__ void stage_row(const float* __restrict__ x, float* s_
     lse = logf(block_reduce<false>(part, sm.w, tid));
 }
 
+// Processing of beam row `beam` (logits row `row`) against history `row`: the token the step fed to that slot joins the history
+// first (each slot is read by exactly one beam row when `append` is given). Returns whether the row's processors are on.
+__device__ __forceinline__ bool beam_proc_begin(const BeamProc& bp, int beam, int row, int V, int tid) {
+    ProcRow& pr = bp.proc.rows[row];
+    const bool on = pr.on != 0;
+    if (on && bp.append != nullptr && tid == 0) {
+        const int t = bp.append[beam], n = pr.hist_len;
+        if (n < bp.proc.cap) {
+            bp.proc.hist[(size_t)row * bp.proc.cap + n] = t;
+            pr.hist_len = n + 1;
+        }
+        if (t >= 0 && t < V) bp.proc.bits[(size_t)row * bp.proc.words + (t >> 5)] |= 1u << (t & 31);
+    }
+    __syncthreads();  // the history and its length are final for process_row
+    return on;
+}
+
+template <bool PROC>
 __global__ void __launch_bounds__(BT_THREADS, 1)
 beam_row_topk_kernel(const float* __restrict__ logits, const int32_t* __restrict__ row_of_beam, const float* __restrict__ beam_scores,
-                     int nb, int V, int K, unsigned long long* __restrict__ keys_out, BeamRowsOut ro) {
+                     int nb, int V, int K, unsigned long long* __restrict__ keys_out, BeamRowsOut ro, BeamProc bp) {
     extern __shared__ __align__(16) uint8_t bt_smem[];
     float* s_x = reinterpret_cast<float*>(bt_smem);
     __shared__ RowSmem sm;
@@ -141,12 +164,30 @@ beam_row_topk_kernel(const float* __restrict__ logits, const int32_t* __restrict
     stage_row(logits + (size_t)row * V, s_x, V, tid, sm, mx, lse);
     const float run = beam_scores[beam];
     const size_t out0 = (size_t)beam * ro.fan * V;
-    for (int i = tid; i < V; i += BT_THREADS) {
-        const float x = s_x[i], ls = (x - mx) - lse;
-        s_x[i] = ls + run;
-        for (int r = 0; r < ro.fan; ++r) {  // output rows: the log-softmax row and the raw row, once per running beam it feeds
-            if (ro.scores != nullptr) ro.scores[out0 + (size_t)r * V + i] = ls;
-            if (ro.logits != nullptr) ro.logits[out0 + (size_t)r * V + i] = x;
+    if constexpr (PROC) {
+        // the log-probabilities, processed in place; the output score row is the processed row
+        for (int i = tid; i < V; i += BT_THREADS) {
+            const float x = s_x[i];
+            s_x[i] = (x - mx) - lse;
+            if (ro.logits != nullptr)
+                for (int r = 0; r < ro.fan; ++r) ro.logits[out0 + (size_t)r * V + i] = x;
+        }
+        if (beam_proc_begin(bp, beam, row, V, tid)) process_row<BT_THREADS>(s_x, V, bp.proc, row, tid);
+        __syncthreads();
+        for (int i = tid; i < V; i += BT_THREADS) {
+            const float ls = s_x[i];
+            s_x[i] = ls + run;
+            if (ro.scores != nullptr)
+                for (int r = 0; r < ro.fan; ++r) ro.scores[out0 + (size_t)r * V + i] = ls;
+        }
+    } else {
+        for (int i = tid; i < V; i += BT_THREADS) {
+            const float x = s_x[i], ls = (x - mx) - lse;
+            s_x[i] = ls + run;
+            for (int r = 0; r < ro.fan; ++r) {  // output rows: the log-softmax row and the raw row, once per running beam it feeds
+                if (ro.scores != nullptr) ro.scores[out0 + (size_t)r * V + i] = ls;
+                if (ro.logits != nullptr) ro.logits[out0 + (size_t)r * V + i] = x;
+            }
         }
     }
     __syncthreads();
@@ -168,11 +209,13 @@ beam_row_topk_kernel(const float* __restrict__ logits, const int32_t* __restrict
 // top-p survivors (at least min_keep of each), the accumulated score acc = w + running score, and for every finite survivor
 // the Gumbel-perturbed key fp32(acc + g), g = -log(-log u) in fp64, u from Philox(seed; step, global flat index). The row's K
 // largest keys are selected as in beam_row_topk_kernel (warped-away tokens are -inf and rank by index below every finite key,
-// NaN logits below them); the candidate's score is its unperturbed acc, written beside its key.
+// NaN logits below them); the candidate's score is its unperturbed acc, written beside its key. With PROC the processors run on
+// the log-probabilities before the division by T.
+template <bool PROC>
 __global__ void __launch_bounds__(BT_THREADS, 1)
 beam_row_sample_kernel(const float* __restrict__ logits, const int32_t* __restrict__ row_of_beam, const float* __restrict__ beam_scores,
                        int nb, int V, int K, BeamSampleParams sp, unsigned long long* __restrict__ keys_out,
-                       float* __restrict__ scores_out, BeamRowsOut ro) {
+                       float* __restrict__ scores_out, BeamRowsOut ro, BeamProc bp) {
     extern __shared__ __align__(16) uint8_t bt_smem[];
     float* s_x = reinterpret_cast<float*>(bt_smem);
     __shared__ RowSmem sm;
@@ -190,7 +233,12 @@ beam_row_sample_kernel(const float* __restrict__ logits, const int32_t* __restri
     const size_t out0 = (size_t)beam * V;  // beam sampling reads one row per running beam: fan is 1
     for (int i = tid; i < V; i += BT_THREADS) {
         if (ro.logits != nullptr) ro.logits[out0 + i] = s_x[i];
-        s_x[i] = __fdiv_rn((s_x[i] - mx) - lse, T);
+        s_x[i] = PROC ? (s_x[i] - mx) - lse : __fdiv_rn((s_x[i] - mx) - lse, T);
+    }
+    if constexpr (PROC) {  // HF's order: processors, then temperature
+        if (beam_proc_begin(bp, beam, row, V, tid)) process_row<BT_THREADS>(s_x, V, bp.proc, row, tid);
+        __syncthreads();
+        for (int i = tid; i < V; i += BT_THREADS) s_x[i] = __fdiv_rn(s_x[i], T);
     }
     __syncthreads();
 
@@ -256,9 +304,16 @@ beam_row_sample_kernel(const float* __restrict__ logits, const int32_t* __restri
         for (int c = 0; c < Kr; ++c) rank += sm.cand[c] > me;
         const int i = (int)(0xFFFFFFFFu - (uint32_t)(me & 0xFFFFFFFFull) - (uint32_t)(j * V));
         const float kx = s_x[i];
-        // a finite key is a survivor: its score is acc, recomputed with the same operations; -inf and NaN carry themselves
+        // a finite key is a survivor: its score is acc, recomputed with the same operations; -inf and NaN carry themselves. A
+        // survivor was not banned by a processor, so of the processors only the repetition penalty can have changed it
+        float w = (x[i] - mx) - lse;
+        if constexpr (PROC) {
+            const ProcRow& pr = bp.proc.rows[row];
+            if (pr.on && pr.penalty != 1.0f && ((bp.proc.bits[(size_t)row * bp.proc.words + (i >> 5)] >> (i & 31)) & 1u))
+                w = repetition_penalised(w, pr.penalty);
+        }
         out[rank] = me;
-        out_s[rank] = (kx == kx && kx > -INFINITY) ? __fdiv_rn((x[i] - mx) - lse, T) + run : kx;
+        out_s[rank] = (kx == kx && kx > -INFINITY) ? __fdiv_rn(w, T) + run : kx;
     } else if (tid < K) {
         out[tid] = 0ull;
         out_s[tid] = -INFINITY;
@@ -315,13 +370,25 @@ kv_copy_slots_kernel(uint8_t* __restrict__ k, uint8_t* __restrict__ v, float* __
     }
 }
 
+__global__ void __launch_bounds__(CP_THREADS) proc_copy_slots_kernel(ProcState proc, KvCopyPairs p) {
+    const int src = p.src[blockIdx.x], dst = p.dst[blockIdx.x];
+    const int n = min(proc.rows[src].hist_len, proc.cap);
+    const int32_t* hs = proc.hist + (size_t)src * proc.cap;
+    int32_t* hd = proc.hist + (size_t)dst * proc.cap;
+    for (int i = threadIdx.x; i < n; i += CP_THREADS) hd[i] = hs[i];
+    const uint32_t* bs = proc.bits + (size_t)src * proc.words;
+    uint32_t* bd = proc.bits + (size_t)dst * proc.words;
+    for (int i = threadIdx.x; i < proc.words; i += CP_THREADS) bd[i] = bs[i];
+    if (threadIdx.x == 0) proc.rows[dst] = proc.rows[src];
+}
+
 }  // namespace
 
 size_t beam_topk_workspace_bytes(int B, int nb, int K) { return (size_t)B * nb * K * sizeof(unsigned long long); }
 
 int beam_topk(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
               void* workspace, float* out_scores, int32_t* out_tokens, int32_t* out_beams, cudaStream_t stream,
-              const BeamRowsOut& rows_out) {
+              const BeamRowsOut& rows_out, const BeamProc& proc) {
     B2_CHECK_ARG(logits && beam_scores && workspace && out_scores && out_tokens && out_beams, "beam_topk: null argument");
     B2_CHECK_ARG(rows_out.fan >= 1, "beam_topk: %d output rows per beam", rows_out.fan);
     B2_CHECK_ARG(B >= 1 && nb >= 1 && nb <= 32, "beam_topk: B=%d nb=%d (1 <= nb <= 32)", B, nb);
@@ -330,13 +397,15 @@ int beam_topk(const float* logits, const int32_t* row_of_beam, const float* beam
     const size_t smem = (size_t)V * sizeof(float);
     B2_CHECK_ARG(V >= 1 && smem <= 200 * 1024 && (long long)nb * V < 0xFFFFFFFFll,
                  "beam_topk: vocab %d exceeds the shared-memory staging of the kernel", V);
-    static size_t attr = 0;
-    if (smem > attr) {
-        B2_CUDA_CHECK(cudaFuncSetAttribute(beam_row_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = smem;
+    const bool on = proc.proc.rows != nullptr;
+    auto* kernel = on ? beam_row_topk_kernel<true> : beam_row_topk_kernel<false>;
+    static size_t attr[2] = {0, 0};
+    if (smem > attr[on]) {
+        B2_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attr[on] = smem;
     }
     auto* keys = reinterpret_cast<unsigned long long*>(workspace);
-    beam_row_topk_kernel<<<dim3(nb, B), BT_THREADS, smem, stream>>>(logits, row_of_beam, beam_scores, nb, V, K, keys, rows_out);
+    kernel<<<dim3(nb, B), BT_THREADS, smem, stream>>>(logits, row_of_beam, beam_scores, nb, V, K, keys, rows_out, proc);
     B2_LAUNCH_CHECK();
     beam_merge_kernel<<<B, BM_THREADS, 0, stream>>>(keys, nullptr, nb, K, V, out_scores, out_tokens, out_beams);
     B2_LAUNCH_CHECK();
@@ -349,7 +418,7 @@ size_t beam_sample_workspace_bytes(int B, int nb, int K) {
 
 int beam_sample(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
                 const BeamSampleParams& sp, void* workspace, float* out_scores, int32_t* out_tokens, int32_t* out_beams,
-                cudaStream_t stream, const BeamRowsOut& rows_out) {
+                cudaStream_t stream, const BeamRowsOut& rows_out, const BeamProc& proc) {
     B2_CHECK_ARG(logits && beam_scores && workspace && out_scores && out_tokens && out_beams, "beam_sample: null argument");
     B2_CHECK_ARG(rows_out.fan == 1, "beam_sample: output rows are written once per beam row (fan %d)", rows_out.fan);
     B2_CHECK_ARG(B >= 1 && nb >= 1 && nb <= 32, "beam_sample: B=%d nb=%d (1 <= nb <= 32)", B, nb);
@@ -362,15 +431,16 @@ int beam_sample(const float* logits, const int32_t* row_of_beam, const float* be
     B2_CHECK_ARG(sp.top_p > 0.f && sp.top_p <= 1.f, "beam_sample: top_p %g outside (0, 1]", (double)sp.top_p);
     B2_CHECK_ARG(sp.top_k >= 0, "beam_sample: top_k %d must be >= 0", sp.top_k);
     B2_CHECK_ARG(sp.min_keep >= 1 && sp.min_keep <= K, "beam_sample: min_keep %d outside [1, K=%d]", sp.min_keep, K);
-    static size_t attr = 0;
-    if (smem > attr) {
-        B2_CUDA_CHECK(cudaFuncSetAttribute(beam_row_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr = smem;
+    const bool on = proc.proc.rows != nullptr;
+    auto* kernel = on ? beam_row_sample_kernel<true> : beam_row_sample_kernel<false>;
+    static size_t attr[2] = {0, 0};
+    if (smem > attr[on]) {
+        B2_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        attr[on] = smem;
     }
     auto* keys = reinterpret_cast<unsigned long long*>(workspace);
     float* scores = reinterpret_cast<float*>(keys + (size_t)B * nb * K);
-    beam_row_sample_kernel<<<dim3(nb, B), BT_THREADS, smem, stream>>>(logits, row_of_beam, beam_scores, nb, V, K, sp, keys, scores,
-                                                                        rows_out);
+    kernel<<<dim3(nb, B), BT_THREADS, smem, stream>>>(logits, row_of_beam, beam_scores, nb, V, K, sp, keys, scores, rows_out, proc);
     B2_LAUNCH_CHECK();
     beam_merge_kernel<<<B, BM_THREADS, 0, stream>>>(keys, scores, nb, K, V, out_scores, out_tokens, out_beams);
     B2_LAUNCH_CHECK();
@@ -391,6 +461,18 @@ int kv_copy_slots(void* k, void* v, float* kscale, float* vscale, const int32_t*
         const dim3 grid((rows + CP_ROWS - 1) / CP_ROWS, L * H * 2, c);
         kv_copy_slots_kernel<<<grid, CP_THREADS, 0, stream>>>(reinterpret_cast<uint8_t*>(k), reinterpret_cast<uint8_t*>(v), kscale, vscale,
                                                                p, row_begin, H, max_batch, pitch, row_bytes, len_dev);
+        B2_LAUNCH_CHECK();
+    }
+    return 0;
+}
+
+int proc_copy_slots(const ProcState& proc, const int32_t* src, const int32_t* dst, int n, cudaStream_t stream) {
+    B2_CHECK_ARG(proc.rows != nullptr && n >= 0, "proc_copy_slots: bad argument");
+    for (int off = 0; off < n; off += KvCopyPairs::kMax) {
+        const int c = n - off < KvCopyPairs::kMax ? n - off : KvCopyPairs::kMax;
+        KvCopyPairs p;
+        for (int i = 0; i < c; ++i) { p.src[i] = src[off + i]; p.dst[i] = dst[off + i]; p.end[i] = 0; }
+        proc_copy_slots_kernel<<<c, CP_THREADS, 0, stream>>>(proc, p);
         B2_LAUNCH_CHECK();
     }
     return 0;

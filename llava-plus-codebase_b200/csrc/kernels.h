@@ -319,9 +319,18 @@ struct BeamRowsOut {
     float* logits = nullptr;
     int fan = 1;
 };
+// Logits processors of beam search (HF's processors over each running beam's log_softmax row, against its own sequence):
+// beam row b*nb + j reads logits row r = row_of_beam[b*nb + j] and, when proc.rows[r].on, first appends append[b*nb + j] to
+// history r (when `append` is non-null), then processes its log-probabilities against history r (process_row) before the
+// running score is added (and, under beam sampling, before the warpers). proc.rows == nullptr: processing off, the kernels of
+// the unprocessed selection run.
+struct BeamProc {
+    ProcState proc = {};
+    const int32_t* append = nullptr;
+};
 int beam_topk(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
               void* workspace, float* out_scores, int32_t* out_tokens, int32_t* out_beams, cudaStream_t stream,
-              const BeamRowsOut& rows_out = BeamRowsOut{});
+              const BeamRowsOut& rows_out = BeamRowsOut{}, const BeamProc& proc = BeamProc{});
 // beam sampling: the same selection over Gumbel-perturbed keys of the warped scores (beam_row_sample_kernel in beam.cu); each
 // candidate's score is its unperturbed accumulated score. T > 0, top_k >= 0 (0 = off), top_p in (0, 1], min_keep >= 1.
 struct BeamSampleParams {
@@ -335,7 +344,7 @@ struct BeamSampleParams {
 size_t beam_sample_workspace_bytes(int B, int nb, int K);
 int beam_sample(const float* logits, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V, int K,
                 const BeamSampleParams& sp, void* workspace, float* out_scores, int32_t* out_tokens, int32_t* out_beams,
-                cudaStream_t stream, const BeamRowsOut& rows_out = BeamRowsOut{});
+                cudaStream_t stream, const BeamRowsOut& rows_out = BeamRowsOut{}, const BeamProc& proc = BeamProc{});
 struct KvCopyPairs {
     static constexpr int kMax = 64;
     int32_t src[kMax], dst[kMax], end[kMax];
@@ -345,6 +354,9 @@ struct KvCopyPairs {
 // No dst may be a src of the same call.
 int kv_copy_slots(void* k, void* v, float* kscale, float* vscale, const int32_t* src, const int32_t* dst, const int32_t* end, int n,
                   int row_begin, int L, int H, int max_batch, int pitch, int row_bytes, int32_t* len_dev, cudaStream_t stream);
+// for each pair i: history row src[i] of `proc` -> row dst[i]: its ProcRow, history ids [0, hist_len) and presence bitmap
+// (one CTA per pair). No dst may be a src of the same call.
+int proc_copy_slots(const ProcState& proc, const int32_t* src, const int32_t* dst, int n, cudaStream_t stream);
 
 // ---- image preprocessing (preprocess.cu): uint8 HWC -> CLIP pixel_values, PIL-exact bicubic resize ------------------------
 struct PreprocessArgs {

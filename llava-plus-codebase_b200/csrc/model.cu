@@ -186,6 +186,12 @@ struct b2_kv {
     DevBuf proc_rows, proc_hist, proc_bits;
     std::vector<char> proc_on;  // host copy of ProcRow::on per slot
     bool any_proc() const { for (char c : proc_on) if (c) return true; return false; }
+    // beam search with logits processors (b2_beam_begin_proc, allocated by its first call): ProcRow[max_batch] of the beams'
+    // cache slots. Their histories and bitmaps share proc_hist / proc_bits (a cache runs one kind of generation at a time), while
+    // the rows stay apart from proc_rows, which every decode step clears and whose rows the decode step's selection would append
+    // its own choice to. Armed until a call turns every row's processors off.
+    DevBuf beam_proc_rows;
+    bool beam_proc_on = false;
     // prompt-lookup speculative decoding (b2_stream_begin_lookup / b2_decode_rows; allocated by the first call): SpecState, the
     // verify forward's logits fp32 [16][V], decode_attn_mq's partials and counters, a mapped host mirror of the step counters,
     // and one captured verify step per row count R. The history lives in proc_hist row 0.
@@ -215,6 +221,11 @@ ProcState proc_state(const b2_kv* kv) {
     if (kv->proc_rows.p == nullptr) return p;
     p.rows = kv->proc_rows.as<ProcRow>(); p.hist = kv->proc_hist.as<int32_t>(); p.bits = kv->proc_bits.as<uint32_t>();
     p.cap = kv->max_seq + 1; p.words = (kv->m->d.vocab + 31) / 32;
+    return p;
+}
+ProcState beam_proc_state(const b2_kv* kv) {
+    ProcState p = proc_state(kv);
+    p.rows = kv->beam_proc_rows.as<ProcRow>();
     return p;
 }
 
@@ -886,7 +897,7 @@ int b2_init(int device) {
 }
 
 const char* b2_last_error(void) { return g_err; }
-int b2_version(void) { return 9; }
+int b2_version(void) { return 10; }
 unsigned long long b2_launch_count(void) { return g_launch_count; }
 
 int b2_model_create(const b2_model_desc* desc, b2_model** out) {
@@ -1347,7 +1358,7 @@ int b2_kv_destroy(b2_kv* kv) {
     DevBuf* bs[] = {&kv->k, &kv->v, &kv->kscale, &kv->vscale, &kv->len_dev, &kv->tok, &kv->step_counter, &kv->out_tokens, &kv->attn_partial,
                     &kv->attn_counters, &kv->mega_layers, &kv->mega_sync, &kv->sk_partial, &kv->sk_counters, &kv->sstate, &kv->rows_dev, &kv->rope_tab,
                     &kv->beam_in, &kv->beam_ws, &kv->beam_out, &kv->proc_rows, &kv->proc_hist, &kv->proc_bits,
-                    &kv->spec_state, &kv->spec_logits, &kv->spec_attn};
+                    &kv->beam_proc_rows, &kv->spec_state, &kv->spec_logits, &kv->spec_attn};
     for (DevBuf* b : bs) b->free();
     delete kv;
     return 0;
@@ -1599,19 +1610,21 @@ static int set_sampling(b2_kv* kv, const SampleState& v, bool force, cudaStream_
     kv->samp_valid = true;
     return 0;
 }
-// every slot selects from its raw logits again (a no-op on a cache whose processors are off)
-static int proc_all_off(b2_kv* kv, cudaStream_t st) {
+// every slot selects from its raw logits again (a no-op on a cache whose processors are off); beam processing is disarmed
+// unless keep_beam (the step of a processed beam search itself)
+static int proc_all_off(b2_kv* kv, cudaStream_t st, bool keep_beam = false) {
+    if (!keep_beam) kv->beam_proc_on = false;
     if (!kv->any_proc()) return 0;
     B2_CUDA_CHECK(cudaMemsetAsync(kv->proc_rows.p, 0, kv->proc_rows.bytes, st));
     kv->proc_on.assign(kv->max_batch, 0);
     return 0;
 }
-static int set_greedy_unpublished(b2_kv* kv, cudaStream_t st) {
+static int set_greedy_unpublished(b2_kv* kv, cudaStream_t st, bool keep_beam = false) {
     SampleState v = {};
     v.temperature = 1.f; v.top_p = 1.f;
     kv->stream_B = 0;  // any streaming generation on this cache is over
     kv->spec_R = 0;
-    B2_TRY(proc_all_off(kv, st));
+    B2_TRY(proc_all_off(kv, st, keep_beam));
     return set_sampling(kv, v, false, st);
 }
 // b2_logits_proc -> ProcRow (on = 0 when every processor is at its off value); prompt ids are checked against `cap`
@@ -1884,6 +1897,80 @@ int b2_op_beam_select_out(const float* logits, const int32_t* row_of_beam, const
     return r;
 }
 
+int b2_op_beam_select_proc(const float* logits, int rows, const int32_t* row_of_beam, const float* beam_scores, int B, int nb, int V,
+                           int K, const b2_beam_sampling* sampling, uint32_t step, int fan, const b2_logits_proc* proc, float* out_scores,
+                           int32_t* out_tokens, int32_t* out_beams, float* row_scores, float* row_logits, void* stream) {
+    B2_CHECK_ARG(B >= 1 && nb >= 1 && nb <= 32 && K >= 1 && K <= 128, "b2_op_beam_select_proc: B=%d nb=%d K=%d", B, nb, K);
+    B2_CHECK_ARG(fan >= 1 && fan <= 32 && (sampling == nullptr || fan == 1),
+                 "b2_op_beam_select_proc: fan %d (1..32, and 1 with sampling)", fan);
+    B2_CHECK_ARG(rows >= 1 && (row_of_beam != nullptr || rows == B * nb), "b2_op_beam_select_proc: %d logits rows for B=%d nb=%d", rows,
+                 B, nb);
+    B2_CHECK_ARG(V >= 1, "b2_op_beam_select_proc: vocab %d", V);
+    // processors: a scratch state whose row r holds proc[r]'s prompt ids as its history
+    std::vector<ProcRow> pr(proc ? rows : 0);
+    int cap = 1;
+    bool any = false;
+    for (int r = 0; r < (int)pr.size(); ++r) {
+        B2_TRY(proc_row_of(proc + r, INT_MAX, &pr[r], "b2_op_beam_select_proc"));
+        cap = std::max(cap, proc[r].prompt_len + 1);
+        any = any || pr[r].on;
+    }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const int words = (V + 31) / 32;
+    const size_t ws_bytes = beam_sample_workspace_bytes(B, nb, K);  // >= beam_topk's
+    const size_t off_rows = (ws_bytes + 255) / 256 * 256, off_hist = off_rows + (size_t)rows * sizeof(ProcRow);
+    const size_t off_bits = off_hist + (size_t)rows * cap * sizeof(int32_t);
+    DevBuf tmp;  // one scratch buffer: the selection's workspace, then (with processors) ProcRow[rows], history [rows][cap], bitmap
+    B2_TRY(tmp.alloc(any ? off_bits + (size_t)rows * words * sizeof(uint32_t) : ws_bytes));
+    BeamProc bp;
+    int r = 0;
+    if (any) {
+        ProcState& ps = bp.proc;
+        ps.rows = reinterpret_cast<ProcRow*>(tmp.as<char>() + off_rows);
+        ps.hist = reinterpret_cast<int32_t*>(tmp.as<char>() + off_hist);
+        ps.bits = reinterpret_cast<uint32_t*>(tmp.as<char>() + off_bits);
+        ps.cap = cap; ps.words = words;
+        if (cudaMemsetAsync(ps.rows, 0, (size_t)rows * sizeof(ProcRow), st) != cudaSuccess) {
+            set_error("b2_op_beam_select_proc: %s", cudaGetErrorString(cudaGetLastError()));
+            r = -2;
+        }
+        for (int i = 0; i < rows && r == 0; ++i)
+            if (pr[i].on) r = proc_seed(ps, i, pr[i], proc[i].prompt_ids, pr[i].prompt_len, -1, V, st);
+    }
+    BeamRowsOut ro;
+    ro.scores = row_scores; ro.logits = row_logits; ro.fan = fan;
+    if (r == 0)
+        r = sampling != nullptr ? beam_sample(logits, row_of_beam, beam_scores, B, nb, V, K, beam_sample_params(sampling, step), tmp.p,
+                                              out_scores, out_tokens, out_beams, st, ro, bp)
+                                : beam_topk(logits, row_of_beam, beam_scores, B, nb, V, K, tmp.p, out_scores, out_tokens, out_beams, st, ro, bp);
+    cudaError_t e = cudaStreamSynchronize(st);
+    tmp.free();
+    if (r != 0) return r;
+    B2_CUDA_CHECK(e);
+    return 0;
+}
+
+int b2_beam_begin_proc(b2_model* m, b2_kv* kv, int B, const b2_logits_proc* proc, void* stream) {
+    B2_CHECK_ARG(m && kv && kv->m == m, "b2_beam_begin_proc: bad handle");
+    B2_CHECK_ARG(B >= 1 && B <= kv->max_batch, "b2_beam_begin_proc: B=%d exceeds the cache's %d slots", B, kv->max_batch);
+    std::vector<ProcRow> pr(B);
+    for (int b = 0; b < B; ++b) B2_TRY(proc_row_of(proc ? proc + b : nullptr, kv->max_seq + 1, &pr[b], "b2_beam_begin_proc"));
+    std::lock_guard<std::mutex> lk(m->mu);
+    DeviceGuard dg(m->device);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    B2_TRY(proc_all_off(kv, st));
+    B2_TRY(proc_alloc(kv, st));
+    if (kv->beam_proc_rows.p == nullptr) B2_TRY(kv->beam_proc_rows.alloc((size_t)kv->max_batch * sizeof(ProcRow)));
+    B2_CUDA_CHECK(cudaMemsetAsync(kv->beam_proc_rows.p, 0, kv->beam_proc_rows.bytes, st));
+    for (int b = 0; b < B; ++b)
+        if (pr[b].on) B2_TRY(proc_seed(beam_proc_state(kv), b, pr[b], proc[b].prompt_ids, pr[b].prompt_len, -1, m->d.vocab, st));
+    kv->beam_proc_on = true;
+    return 0;
+}
+
+static int beam_step(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, const b2_beam_sampling* sampling, uint32_t step,
+                     float* row_scores, float* row_logits, bool proc, void* stream);
+
 int b2_beam_step(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, void* stream) {
     return b2_beam_step_ex(m, kv, a, nullptr, 0u, stream);
 }
@@ -1894,6 +1981,16 @@ int b2_beam_step_ex(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, const b2
 
 int b2_beam_step_out(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, const b2_beam_sampling* sampling, uint32_t step,
                      float* row_scores, float* row_logits, void* stream) {
+    return beam_step(m, kv, a, sampling, step, row_scores, row_logits, false, stream);
+}
+
+int b2_beam_step_proc(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, const b2_beam_sampling* sampling, uint32_t step,
+                      float* row_scores, float* row_logits, void* stream) {
+    return beam_step(m, kv, a, sampling, step, row_scores, row_logits, true, stream);
+}
+
+static int beam_step(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, const b2_beam_sampling* sampling, uint32_t step,
+                     float* row_scores, float* row_logits, bool proc, void* stream) {
     B2_CHECK_ARG(m && kv && a && kv->m == m, "b2_beam_step: bad handle");
     B2_CHECK_ARG(m->finalized, "b2_beam_step: model not finalized");
     const int B = a->B, nb = a->nb, K = a->K, n = a->B * a->nb;
@@ -1911,6 +2008,7 @@ int b2_beam_step_out(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, const b
     std::lock_guard<std::mutex> lk(m->mu);
     DeviceGuard dg(m->device);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    B2_CHECK_ARG(!proc || kv->beam_proc_on, "b2_beam_step_proc: beam processing is not armed on this cache (b2_beam_begin_proc)");
     std::vector<int32_t> end;
     B2_TRY(check_copies(kv, a->copy_src_host, a->copy_dst_host, a->n_copies, a->row_begin, end));
     std::vector<int32_t> len(kv->len_host.begin(), kv->len_host.begin() + n), tok(n, -1);
@@ -1926,15 +2024,17 @@ int b2_beam_step_out(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, const b
         B2_CHECK_ARG(len[s] >= 1 && len[s] < kv->max_seq, "b2_beam_step: slot %d has cache length %d (capacity %d)", s, len[s],
                      kv->max_seq);
     if (kv->beam_in.p == nullptr) {
-        B2_TRY(kv->beam_in.alloc((size_t)2 * kv->max_batch * 4));
+        B2_TRY(kv->beam_in.alloc((size_t)3 * kv->max_batch * 4));
         B2_TRY(kv->beam_ws.alloc(beam_sample_workspace_bytes(kv->max_batch, 1, 128)));  // >= beam_topk's
         B2_TRY(kv->beam_out.alloc((size_t)kv->max_batch * 128 * 12));
     }
     B2_TRY(ws_enter(m, st));
     B2_TRY(launch_copies(m, kv, a->copy_src_host, a->copy_dst_host, end, a->n_copies, a->row_begin, st));
+    // a copied slot takes its source's history with its K/V rows (the whole history: it is in token space, not cache rows)
+    if (proc && a->n_copies > 0) B2_TRY(proc_copy_slots(beam_proc_state(kv), a->copy_src_host, a->copy_dst_host, a->n_copies, st));
     B2_TRY(copy_tokens_in(kv, tok.data(), n, st));
     B2_CUDA_CHECK(cudaMemsetAsync(kv->step_counter.p, 0, 4, st));
-    B2_TRY(set_greedy_unpublished(kv, st));
+    B2_TRY(set_greedy_unpublished(kv, st, proc));
     cudaStream_t run = nullptr;
     B2_TRY(fork_stream(kv, st, &run));
     B2_TRY(decode_step_run(m, kv, n, run));
@@ -1948,11 +2048,18 @@ int b2_beam_step_out(b2_model* m, b2_kv* kv, const b2_beam_step_args* a, const b
     const float* run_scores = reinterpret_cast<const float*>(rows + kv->max_batch);
     BeamRowsOut ro;
     ro.scores = row_scores; ro.logits = row_logits;
+    BeamProc bp;
+    if (proc) {  // each beam's token joins its slot's history inside the row kernel, before the row is processed
+        int32_t* append = rows + 2 * kv->max_batch;
+        B2_TRY(set_i32_pairs(append, a->tokens_host, nullptr, nullptr, n, st));
+        bp.proc = beam_proc_state(kv);
+        bp.append = append;
+    }
     if (sampling != nullptr)
         B2_TRY(beam_sample(m->logits.as<float>(), rows, run_scores, B, nb, m->d.vocab, K, beam_sample_params(sampling, step), kv->beam_ws.p,
-                           o_s, o_t, o_b, st, ro));
+                           o_s, o_t, o_b, st, ro, bp));
     else
-        B2_TRY(beam_topk(m->logits.as<float>(), rows, run_scores, B, nb, m->d.vocab, K, kv->beam_ws.p, o_s, o_t, o_b, st, ro));
+        B2_TRY(beam_topk(m->logits.as<float>(), rows, run_scores, B, nb, m->d.vocab, K, kv->beam_ws.p, o_s, o_t, o_b, st, ro, bp));
     B2_CUDA_CHECK(cudaMemcpyAsync(a->out_scores_host, o_s, (size_t)B * K * 4, cudaMemcpyDeviceToHost, st));
     B2_CUDA_CHECK(cudaMemcpyAsync(a->out_tokens_host, o_t, (size_t)B * K * 4, cudaMemcpyDeviceToHost, st));
     B2_CUDA_CHECK(cudaMemcpyAsync(a->out_beams_host, o_b, (size_t)B * K * 4, cudaMemcpyDeviceToHost, st));

@@ -20,6 +20,7 @@
 
 #include "common.cuh"
 #include "kernels.h"
+#include "logits_proc.cuh"
 #include "select.cuh"
 
 namespace b2 {
@@ -57,38 +58,6 @@ __device__ __forceinline__ int block_argmax(const float* row, int V, int tid, fl
     }
     if (max_out) *max_out = best;
     return bi == INT_MAX ? 0 : bi;
-}
-
-// HF's history-aware processors over the staged row s_x, in transformers' order (repetition -> no-repeat-ngram -> min_length /
-// min_new_tokens). Ids of the history outside [0, V) (IMAGE_TOKEN_INDEX placeholders) are never penalised or banned.
-__device__ __forceinline__ void process_row(float* s_x, int V, const ProcState& proc, int b, int tid) {
-    const ProcRow& pr = proc.rows[b];
-    const int L = pr.hist_len, n = pr.ngram;
-    const float p = pr.penalty;
-    const int32_t* hist = proc.hist + (size_t)b * proc.cap;
-    const uint32_t* bits = proc.bits + (size_t)b * proc.words;
-    __syncthreads();  // the staged row is complete
-    if (p != 1.0f) {  // RepetitionPenaltyLogitsProcessor: once per distinct id of the history, IEEE fp32
-        for (int i = tid; i < V; i += SP_THREADS)
-            if ((bits[i >> 5] >> (i & 31)) & 1u) {
-                const float x = s_x[i];
-                s_x[i] = x < 0.f ? __fmul_rn(x, p) : __fdiv_rn(x, p);
-            }
-        __syncthreads();
-    }
-    if (n > 0 && L + 1 >= n) {  // NoRepeatNGramLogitsProcessor: every n-gram whose first n-1 ids equal the last n-1 ids
-        const int32_t* tail = hist + (L - n + 1);
-        for (int s = tid; s <= L - n; s += SP_THREADS) {
-            bool match = true;
-            for (int j = 0; j < n - 1 && match; ++j) match = hist[s + j] == tail[j];
-            const int t = hist[s + n - 1];
-            if (match && t >= 0 && t < V) s_x[t] = -INFINITY;  // idempotent: threads may ban the same id
-        }
-    }
-    if (L - pr.prompt_len < pr.min_gen && tid < pr.n_eos) {  // MinLength / MinNewTokensLength
-        const int e = pr.eos[tid];
-        if (e >= 0 && e < V) s_x[e] = -INFINITY;
-    }
 }
 
 // HF 5.5 assisted decoding's acceptance (generation/utils.py, n_matches): the draft's leading tokens that equal the tokens
@@ -178,7 +147,7 @@ sample_publish_kernel(const float* __restrict__ logits, int V, int B, SampleStat
     if (select && (proc_on || processed_out != nullptr)) {
         // stage the row and run the processors in HF's order over it; selection below reads the staged row
         for (int i = tid; i < V; i += SP_THREADS) s_x[i] = row[i];
-        if (proc_on) process_row(s_x, V, proc, b, tid);
+        if (proc_on) process_row<SP_THREADS>(s_x, V, proc, b, tid);
         __syncthreads();
         if (processed_out != nullptr)
             for (int i = tid; i < V; i += SP_THREADS) processed_out[(size_t)b * V + i] = s_x[i];

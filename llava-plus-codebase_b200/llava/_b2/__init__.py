@@ -198,6 +198,10 @@ SIGNATURES = {
     "b2_op_beam_select_out": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _c.POINTER(BeamSampling), _c.c_uint32, _i32, _vp, _vp,
                                      _vp, _vp, _vp, _vp]),
     "b2_beam_step_out": (_i32, [_vp, _vp, _c.POINTER(BeamStepArgs), _c.POINTER(BeamSampling), _c.c_uint32, _vp, _vp, _vp]),
+    "b2_op_beam_select_proc": (_i32, [_vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _c.POINTER(BeamSampling), _c.c_uint32, _i32,
+                                      _c.POINTER(LogitsProc), _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b2_beam_begin_proc": (_i32, [_vp, _vp, _i32, _c.POINTER(LogitsProc), _vp]),
+    "b2_beam_step_proc": (_i32, [_vp, _vp, _c.POINTER(BeamStepArgs), _c.POINTER(BeamSampling), _c.c_uint32, _vp, _vp, _vp]),
     "b2_op_gemm": (_i32, [_vp, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "b2_op_gemv": (_i32, [_vp, _i64, _vp, _i32, _vp, _f32, _vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
     "b2_op_quantize_nf4": (_i32, [_vp, _i32, _i32, _vp, _vp, _vp]),
@@ -670,8 +674,46 @@ class Engine:
                   "b2_op_beam_select_out")
         return out_s, out_t, out_b
 
+    def beam_select_proc(self, logits, beam_scores, nb, K, procs, row_scores=None, row_logits=None, sampling=None, step=0,
+                         row_of_beam=None, fan=1):
+        """beam_select_out with logits processors (b2_op_beam_select_proc): `procs` holds one LogitsProc (or None) per logits row,
+        processing that row's log-probabilities against its prompt ids. Returns device tensors (scores fp32, tokens int32, beams
+        int32), each [B, K]; synchronises."""
+        V = logits.shape[-1]
+        rows_n = logits.numel() // V
+        scores = beam_scores.to(device=self.device, dtype=torch.float32).contiguous()
+        B = scores.numel() // nb
+        rows = None if row_of_beam is None else torch.as_tensor(row_of_beam, dtype=torch.int32).to(self.device).contiguous()
+        for o in (row_scores, row_logits):
+            if o is not None and (o.dtype != torch.float32 or o.numel() != B * nb * fan * V or not o.is_contiguous()):
+                raise ValueError(f"output rows must be contiguous fp32 [{B * nb * fan}, {V}]")
+        arr = _proc_array(procs, rows_n)
+        out_s = torch.empty(B, K, dtype=torch.float32, device=self.device)
+        out_t = torch.empty(B, K, dtype=torch.int32, device=self.device)
+        out_b = torch.empty(B, K, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.index):
+            check(self.lib.b2_op_beam_select_proc(ptr(logits), rows_n, ptr(rows), ptr(scores), B, int(nb), V, int(K),
+                                                  None if sampling is None else ctypes.byref(sampling), int(step), int(fan), arr,
+                                                  ptr(out_s), ptr(out_t), ptr(out_b), ptr(row_scores), ptr(row_logits), stream_ptr()),
+                  "b2_op_beam_select_proc")
+        return out_s, out_t, out_b
+
+    def beam_begin_proc(self, kv, procs):
+        """Arms the logits processors of a beam search on `kv` (b2_beam_begin_proc): slot b gets procs[b] (LogitsProc or None),
+        its history seeded from the prompt ids; b2_beam_step_proc (beam_step_proc) then processes every beam against its slot's
+        history."""
+        arr = _proc_array(procs, len(procs))
+        with torch.cuda.device(self.index):
+            check(self.lib.b2_beam_begin_proc(self.handle, kv.handle, len(procs), arr, stream_ptr()), "b2_beam_begin_proc")
+
+    def beam_step_proc(self, kv, copies, row_begin, tokens, slot_of_beam, beam_scores, nb, K, sampling=None, step=0,
+                       row_scores=None, row_logits=None):
+        """beam_step with the processors armed by beam_begin_proc (b2_beam_step_proc)."""
+        return self.beam_step(kv, copies, row_begin, tokens, slot_of_beam, beam_scores, nb, K, sampling, step, row_scores,
+                              row_logits, _proc=True)
+
     def beam_step(self, kv, copies, row_begin, tokens, slot_of_beam, beam_scores, nb, K, sampling=None, step=0, row_scores=None,
-                  row_logits=None):
+                  row_logits=None, _proc=False):
         """One step of the running beams (b2_beam_step, or b2_beam_step_ex with a BeamSampling): `copies` = [(src, dst)] applied
         first, tokens[i] fed to slot slot_of_beam[i], one decode step at batch len(tokens), candidates of every sample selected
         (or, with `sampling`, drawn as draw `step`) on the device. Returns CPU tensors (scores fp32, tokens int64, beams int64),
@@ -690,10 +732,14 @@ class Engine:
                          _c.cast(slots, _vp), _c.cast(scores, _vp), _vp(out_s.data_ptr()), _vp(out_t.data_ptr()),
                          _vp(out_b.data_ptr()))
         with torch.cuda.device(self.index):
-            if row_scores is not None or row_logits is not None:
-                for o in (row_scores, row_logits):
-                    if o is not None and (o.dtype != torch.float32 or o.numel() != n * self.vocab or not o.is_contiguous()):
-                        raise ValueError(f"output rows must be contiguous fp32 [{n}, {self.vocab}]")
+            for o in (row_scores, row_logits):
+                if o is not None and (o.dtype != torch.float32 or o.numel() != n * self.vocab or not o.is_contiguous()):
+                    raise ValueError(f"output rows must be contiguous fp32 [{n}, {self.vocab}]")
+            if _proc:
+                check(self.lib.b2_beam_step_proc(self.handle, kv.handle, ctypes.byref(a),
+                                                 None if sampling is None else ctypes.byref(sampling), int(step), ptr(row_scores),
+                                                 ptr(row_logits), stream_ptr()), "b2_beam_step_proc")
+            elif row_scores is not None or row_logits is not None:
                 check(self.lib.b2_beam_step_out(self.handle, kv.handle, ctypes.byref(a),
                                                 None if sampling is None else ctypes.byref(sampling), int(step), ptr(row_scores),
                                                 ptr(row_logits), stream_ptr()), "b2_beam_step_out")

@@ -520,9 +520,10 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         proc_args = self._logits_processor_arguments(kwargs)
         beam_args = {}
         if num_beams != 1:
-            if proc_args:
+            if proc_args and not _beam_logits_processors_on(self.config):
                 raise NotImplementedError("logits processors (repetition_penalty, no_repeat_ngram_size, min_new_tokens, "
-                                          "min_length) together with num_beams > 1 are not implemented on the H100 path")
+                                          "min_length) together with num_beams > 1 are not implemented on the H100 path "
+                                          "without config.b2_beam_logits_processors")
             if self._beam_search_cap() < 2:
                 raise NotImplementedError("beam search is not used on the LLaVA path (num_beams=1 everywhere)")
             beam_args = self._beam_arguments(num_beams, do_sample, temperature, top_p, top_k, streamer, kwargs)
@@ -551,11 +552,20 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             max_new_tokens = (max_length - Lt) if max_length is not None else 20
         if max_new_tokens <= 0:
             raise ValueError("max_new_tokens must be positive")
+        procs = None
+        if proc_args:
+            # history of row b = the prompt row as passed (placeholders and pad ids included), kept on the device
+            prompt_dev = prompt.to(device=engine.device, dtype=torch.int64).contiguous()
+            procs = [make_logits_proc(prompt_dev[b], proc_args["repetition_penalty"], proc_args["no_repeat_ngram_size"],
+                                      max(proc_args["min_new_tokens"], proc_args["min_length"] - Lt), eos_ids)
+                     for b in range(B)]
+            if all(p is None for p in procs):
+                procs = None
         if beam_args:
             eos_list = (list(eos_token_id) if isinstance(eos_token_id, (list, tuple))
                         else (None if eos_token_id is None else [eos_token_id]))
             return self._beam_generate(engine, prompt, images, attention_mask, num_beams, max_new_tokens, eos_list, pad_token_id,
-                                       stopping_criteria, want=want, **beam_args)
+                                       stopping_criteria, want=want, procs=procs, **beam_args)
         greedy = (not do_sample) or (temperature is not None and temperature <= 1e-5)
         if greedy:
             sampling = make_sampling()
@@ -566,15 +576,6 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             # torch.manual_seed() makes a run repeatable
             seed = int(torch.randint(0, 2**62, (1,), dtype=torch.int64).item())
             sampling = make_sampling(True, temperature, 1.0 if top_p is None else top_p, 50 if top_k is None else top_k, seed)
-        procs = None
-        if proc_args:
-            # history of row b = the prompt row as passed (placeholders and pad ids included), kept on the device
-            prompt_dev = prompt.to(device=engine.device, dtype=torch.int64).contiguous()
-            procs = [make_logits_proc(prompt_dev[b], proc_args["repetition_penalty"], proc_args["no_repeat_ngram_size"],
-                                      max(proc_args["min_new_tokens"], proc_args["min_length"] - Lt), eos_ids)
-                     for b in range(B)]
-            if all(p is None for p in procs):
-                procs = None
         lookup = None  # prompt-lookup speculative decoding (batch 1): lookup(cache rows) -> PromptLookup, or None when K rows no longer fit
         if lookup_args and self._get_batcher(engine) is None:
             def lookup(rows):
@@ -841,7 +842,7 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                     num_return_sequences=1 if nrs is None else int(nrs), sampling=sampling)
 
     def _beam_generate(self, engine, prompt, images, attention_mask, num_beams, max_new_tokens, eos_ids, pad_token_id,
-                       stopping_criteria, length_penalty, early_stopping, num_return_sequences, sampling=None, want=None):
+                       stopping_criteria, length_penalty, early_stopping, num_return_sequences, sampling=None, want=None, procs=None):
         """Beam search (llava/_b2/beam.py): sample b is prefilled once into slot b of a pool cache; its candidates from the
         prefill logits fork the prompt into nb slots; then every b2_beam_step applies the step's slot copies, decodes the
         B * nb running beams in one batch and returns the K best candidates per sample for the host bookkeeping.
@@ -852,7 +853,14 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         the list when fewer than K have positive probability.
 
         `want` (generate()'s _output_arguments): the device also writes each step's score and raw logits rows, [B * nb, V] in
-        running-beam order, and the result is a GenerateBeamDecoderOnlyOutput."""
+        running-beam order, and the result is a GenerateBeamDecoderOnlyOutput.
+
+        `procs` (config.b2_beam_logits_processors): one LogitsProc (or None) per sample. Each running beam's log-probabilities are
+        processed against its own sequence, as HF's _beam_search does: the first candidates come from the prefill row processed
+        over the prompt (b2_op_beam_select_proc), then b2_beam_begin_proc gives slot b sample b's processors and prompt history,
+        and every b2_beam_step_proc carries the histories along the slot copies and appends each step's tokens. The host
+        bookkeeping is unchanged: the candidates' scores are already the processed accumulated scores, and the score rows the
+        processed (warped) rows."""
         from ..._b2 import beam as _beam
 
         B = prompt.shape[0]
@@ -878,7 +886,18 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 self._check_limits(engine, B * nb, max(lens) + max_new_tokens)
                 kv.reset()
                 logits = engine.prefill(kv, embeds, lens, LOGITS_LAST)
-                if want:  # the same selection, also writing step 0's rows (the one prefill row of a sample fills its nb rows)
+                if procs is not None:  # processed over each sample's prompt; a sample's prefill row feeds all of its beams
+                    if bs is None:
+                        cand = engine.beam_select_proc(logits, torch.zeros(B), 1, search.K, procs, at("scores", 0), at("logits", 0),
+                                                       fan=nb)
+                    else:
+                        cand = engine.beam_select_proc(logits, search.running_scores.reshape(-1), nb, search.K, procs, at("scores", 0),
+                                                       at("logits", 0), sampling=bs, step=0,
+                                                       row_of_beam=[b for b in range(B) for _ in range(nb)])
+                    cand = [t.cpu() for t in cand]
+                    if bs is not None:
+                        cand[2].zero_()
+                elif want:  # the same selection, also writing step 0's rows (the one prefill row of a sample fills its nb rows)
                     if bs is None:
                         cand = engine.beam_select_out(logits, torch.zeros(B), 1, search.K, at("scores", 0), at("logits", 0), fan=nb)
                     else:
@@ -903,13 +922,17 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 err = engine.take_async_error()
             if err:
                 raise ValueError(last_error())
+            beam_step = engine.beam_step
+            if procs is not None:
+                engine.beam_begin_proc(kv, procs)
+                beam_step = engine.beam_step_proc
             planner = _beam.SlotPlanner(B, nb)
             row_begin = 0  # the first plan copies whole prompts; later ones only rows behind the shortest prompt
             step = 0
             while not search.step(*cand):
                 step += 1
                 copies = planner.plan(search.parents)
-                cand = engine.beam_step(kv, copies, row_begin, search.next_tokens().tolist(), planner.flat(),
+                cand = beam_step(kv, copies, row_begin, search.next_tokens().tolist(), planner.flat(),
                                         search.running_scores.reshape(-1).tolist(), nb, search.K, sampling=bs, step=step,
                                         **({"row_scores": at("scores", step), "row_logits": at("logits", step)} if want else {}))
                 row_begin = min(lens)
@@ -1045,6 +1068,13 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
 
     def eval(self):
         return super().eval()
+
+
+def _beam_logits_processors_on(config):
+    """config.b2_beam_logits_processors or B2_BEAM_LOGITS_PROCESSORS=1: generate(num_beams > 1) runs the logits processors that
+    config.b2_logits_processors enables (off by default, like the other b2_* opt-ins)."""
+    v = getattr(config, "b2_beam_logits_processors", None)
+    return bool(v) if v is not None else os.environ.get("B2_BEAM_LOGITS_PROCESSORS") == "1"
 
 
 def _nf4_requested(kwargs):
