@@ -232,6 +232,28 @@ int b2_stream_begin(b2_model* m, b2_kv* kv, const float* logits, int B, const b2
  * than the cache's max_seq. */
 int b2_stream_begin_ex(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sampling, const b2_logits_proc* proc,
                        void* stream);
+/* Shared-prefix decode of forked samples (generate(num_return_sequences=n)): rows that hold copies of one prompt's cache rows
+ * (b2_kv_copy_slots) form a group, and while the group table is armed the decode attention reads keys [0, prefix_len) of every
+ * row of a group once, from the group's source slot, instead of once per row from the row's own copy. The result is the one the
+ * rows' own copies give, up to the order of floating-point sums.
+ *   src_slot    the slot whose rows [0, prefix_len) the group's rows read;
+ *   prefix_len  1 <= prefix_len <= the current length of src_slot and of every member row;
+ *   rows        n_rows (1..16) rows of the batch; a row belongs to at most one group, and rows outside every group attend their
+ *               own slot only. Split more than 16 rows of a prompt into several groups naming the same source. */
+typedef struct {
+    int32_t src_slot;
+    int32_t prefix_len;
+    int32_t n_rows;
+    int32_t rows[16];
+} b2_prefix_group;
+/* b2_stream_begin_ex that also arms `groups[0..G)` (G in 1..B, src_slot < B) for the decode steps of this generation. -1 (nothing
+ * queued) for a table that breaks the rules above. The table's device state is allocated by the first call (b2_kv_bytes does not
+ * count it). Only the multi-kernel decode step over a bf16 cache reads the table: the megakernel (batch <= 2) and an e4m3
+ * cache read every row's own copy. Every other call that begins a generation or decodes on the cache (b2_stream_begin*,
+ * b2_stream_begin_lookup, b2_batch_begin, b2_decode_step, b2_decode_greedy, b2_decode_rows, b2_beam_step*) and b2_kv_reset
+ * disarm it. Arming or disarming drops the cache's captured decode graph. */
+int b2_stream_begin_groups(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sampling, const b2_logits_proc* proc,
+                           const b2_prefix_group* groups, int G, void* stream);
 int b2_stream_enqueue(b2_model* m, b2_kv* kv, int n_steps, void* stream);
 int b2_stream_wait(b2_kv* kv, int index, int32_t* tokens_host, int timeout_ms);
 /* Score and logits rows of a streaming generation (generate(output_scores / output_logits, return_dict_in_generate)).
@@ -464,6 +486,15 @@ int b2_op_decode_attn_mq(const void* qkv, const void* kcache, const void* vcache
 int64_t b2_op_decode_attn_mq_scratch_bytes(int B, int H, int nsplit);
 /* the split factor the verify step uses for b2_op_decode_attn_mq at H heads and a cache of Smax rows (from the kernel's occupancy) */
 int b2_op_decode_attn_mq_nsplit(int H, int Smax);
+/* b2_op_decode_attn with the group table `groups_host` (host, G groups, the rules of b2_prefix_group; prefix_len is checked against
+ * Smax only, the caller keeps it <= cur_len of the source and of every member): row b's keys [0, prefix_len) come from its group's
+ * source slot. The table is copied into `scratch` (b2_op_decode_attn_shared_scratch_bytes, zero-filled once); synchronises. */
+int b2_op_decode_attn_shared(const void* qkv, void* kcache, void* vcache, const int32_t* cur_len, const b2_prefix_group* groups_host,
+                             int G, void* out, void* scratch, int B, int H, int Smax, int nsplit, float theta, float scale,
+                             void* stream);
+int64_t b2_op_decode_attn_shared_scratch_bytes(int B, int H, int nsplit);
+/* the split factor the decode step uses for b2_op_decode_attn_shared at B rows, H heads and a cache of Smax rows */
+int b2_op_decode_attn_shared_nsplit(int B, int H, int Smax);
 /* the draft of one prompt-lookup step: hist device int32 [len] (the last id is the pending token), max_length = prompt length +
  * max_new_tokens of the generation; out_tokens device int32 [num_tokens + 1] = pending, draft, padding; out_draft_len device int32.
  * Synchronises the stream. */

@@ -149,30 +149,27 @@ struct DecodeAttnParams {
     float theta, scale_log2;
 };
 
-__global__ void __launch_bounds__(DA_THREADS) decode_attn_kernel(DecodeAttnParams p) {
-    const int split = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
+// One CTA of decode attention for sample b, head `head`: RoPE of q and of the new k at pos, the append of the new K / V row when
+// this split's range holds pos, and the half-warp attention over keys [key_lo + split * chunk, ...) of [key_lo, pos] in b's slab;
+// this CTA's partial (o[128], m, l) goes to slot part_off + split of the part_stride slots of (b, head). decode_attn_kernel runs it over [0, pos], the shared-prefix
+// kernel over a row's suffix [P, pos]: both append bit-identical rows.
+__device__ __forceinline__ void decode_attn_cta(const __nv_bfloat16* qkv, __nv_bfloat16* kcache, __nv_bfloat16* vcache, int b,
+                                                int head, int split, int nsplit, int pos, int key_lo, int H, int Smax, float theta,
+                                                float scale_log2, float* partial, int part_stride, int part_off, float* s_q, float* s_knew, float* s_m, float* s_l,
+                                                float (*s_o)[DA_D]) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int hw = (warp << 1) | (lane >> 4);  // half-warp id 0..7
     const int c = lane & 15;                   // 8-element chunk of the head dim
-    pdl_trigger();
-    pdl_wait();                                // qkv (previous GEMM) and cur_len (previous step) are upstream outputs
-    const int pos = p.cur_len[b];              // position of the new token == number of cached keys
     const int total = pos + 1;
-    const int hd = p.H * DA_D;
-
-    __shared__ float s_q[DA_D];
-    __shared__ float s_knew[DA_D];
-    __shared__ float s_m[8], s_l[8];
-    __shared__ float s_o[8][DA_D];
-    __shared__ int s_last;
+    const int hd = H * DA_D;
 
     // ---- RoPE on q and the new k (every CTA: 128 threads, one element each) ----
     {
-        const __nv_bfloat16* qrow = p.qkv + (size_t)b * 3 * hd + head * DA_D;
+        const __nv_bfloat16* qrow = qkv + (size_t)b * 3 * hd + head * DA_D;
         const __nv_bfloat16* krow = qrow + hd;
         const int i = tid & 63;
         float cs, sn;
-        rope_cos_sin(pos, i, DA_D, p.theta, cs, sn);
+        rope_cos_sin(pos, i, DA_D, theta, cs, sn);
         const float q1 = __bfloat162float(qrow[i]), q2 = __bfloat162float(qrow[i + 64]);
         const float k1 = __bfloat162float(krow[i]), k2 = __bfloat162float(krow[i + 64]);
         if (tid < 64) {
@@ -186,17 +183,17 @@ __global__ void __launch_bounds__(DA_THREADS) decode_attn_kernel(DecodeAttnParam
     __syncthreads();
 
     // key range of this split (device-side: the launch grid is fixed so the step can live in a CUDA graph)
-    const int chunk = (total + p.nsplit - 1) / p.nsplit;
-    const int k_begin = split * chunk;
+    const int chunk = (total - key_lo + nsplit - 1) / nsplit;
+    const int k_begin = key_lo + split * chunk;
     const int k_end = min(k_begin + chunk, total);
     const bool owns_new = (pos >= k_begin) && (pos < k_end);
 
-    const size_t cbase = ((size_t)b * p.H + head) * p.Smax * DA_D;
+    const size_t cbase = ((size_t)b * H + head) * Smax * DA_D;
     if (owns_new) {
         // append the new token's k (roped) and v to the cache; exactly one CTA per (b, head) does this
-        const __nv_bfloat16* vrow = p.qkv + (size_t)b * 3 * hd + 2 * hd + head * DA_D;
-        p.kcache[cbase + (size_t)pos * DA_D + tid] = __float2bfloat16_rn(s_knew[tid]);
-        p.vcache[cbase + (size_t)pos * DA_D + tid] = vrow[tid];
+        const __nv_bfloat16* vrow = qkv + (size_t)b * 3 * hd + 2 * hd + head * DA_D;
+        kcache[cbase + (size_t)pos * DA_D + tid] = __float2bfloat16_rn(s_knew[tid]);
+        vcache[cbase + (size_t)pos * DA_D + tid] = vrow[tid];
     }
 
     float qreg[8];
@@ -208,10 +205,9 @@ __global__ void __launch_bounds__(DA_THREADS) decode_attn_kernel(DecodeAttnParam
 #pragma unroll
     for (int e = 0; e < 8; ++e) acc[e] = 0.f;
 
-    const __nv_bfloat16* kb = p.kcache + cbase + c * 8;
-    const __nv_bfloat16* vb = p.vcache + cbase + c * 8;
-    const __nv_bfloat16* vnew = p.qkv + (size_t)b * 3 * hd + 2 * hd + head * DA_D + c * 8;
-
+    const __nv_bfloat16* kb = kcache + cbase + c * 8;
+    const __nv_bfloat16* vb = vcache + cbase + c * 8;
+    const __nv_bfloat16* vnew = qkv + (size_t)b * 3 * hd + 2 * hd + head * DA_D + c * 8;
     // each half-warp walks keys k_begin + hw, +8, ...; DA_UNROLL keys (2*DA_UNROLL 16B loads) in flight
     // (trip count is CTA-uniform: the shuffles below use the full warp mask)
     for (int kbase = k_begin; kbase < k_end; kbase += 8 * DA_UNROLL) {
@@ -257,7 +253,7 @@ __global__ void __launch_bounds__(DA_THREADS) decode_attn_kernel(DecodeAttnParam
             dot += __shfl_xor_sync(0xffffffffu, dot, 2);
             dot += __shfl_xor_sync(0xffffffffu, dot, 1);
             if (valid) {
-                const float sc = dot * p.scale_log2;
+                const float sc = dot * scale_log2;
                 const float m_new = fmaxf(m_run, sc);
                 const float corr = exp2f(m_run - m_new);
                 const float pr = exp2f(sc - m_new);
@@ -284,10 +280,29 @@ __global__ void __launch_bounds__(DA_THREADS) decode_attn_kernel(DecodeAttnParam
         l_cta += s_l[i] * w;
         o_cta += s_o[i][tid] * w;
     }
-    const int bh = b * p.H + head;
-    float* part = p.partial + ((size_t)bh * p.nsplit + split) * (DA_D + 2);
+    const int bh = b * H + head;
+    float* part = partial + ((size_t)bh * part_stride + part_off + split) * (DA_D + 2);
     part[tid] = o_cta;
     if (tid == 0) { part[DA_D] = m_cta; part[DA_D + 1] = l_cta; }
+}
+
+__global__ void __launch_bounds__(DA_THREADS) decode_attn_kernel(DecodeAttnParams p) {
+    const int split = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
+    const int tid = threadIdx.x;
+    pdl_trigger();
+    pdl_wait();                                // qkv (previous GEMM) and cur_len (previous step) are upstream outputs
+    const int pos = p.cur_len[b];              // position of the new token == number of cached keys
+    const int hd = p.H * DA_D;
+
+    __shared__ float s_q[DA_D];
+    __shared__ float s_knew[DA_D];
+    __shared__ float s_m[8], s_l[8];
+    __shared__ float s_o[8][DA_D];
+    __shared__ int s_last;
+
+    decode_attn_cta(p.qkv, p.kcache, p.vcache, b, head, split, p.nsplit, pos, 0, p.H, p.Smax, p.theta, p.scale_log2, p.partial,
+                    p.nsplit, 0, s_q, s_knew, s_m, s_l, s_o);
+    const int bh = b * p.H + head;
 
     // ---- last CTA of this (b, head) merges the splits ----
     __threadfence();
@@ -540,6 +555,278 @@ __global__ void __launch_bounds__(128) decode_attn_mq_kernel(DecodeAttnMqParams 
             p.out[((size_t)b * R + r) * hd + head * DA_D + tid] = __float2bfloat16_rn(o_all / l_all);
         }
         if (tid == 0) p.counters[bh] = 0;  // self-reset for the next launch
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// shared-prefix decode attention: the result of decode_attn_kernel for every row b at pos = cur_len[b], for a batch whose rows
+// come in groups that share a prompt. Keys [0, P_g) of group g's rows are read from the group's source slot (the rows' own
+// copies of them are never read); keys [P_g, pos] of a row come from its own slot, and a row outside every group attends its
+// own slot only. grid (nsplit, H, G + B), 128 threads:
+//   z <  G : group z's prefix, split nsplit ways. Each 64-key tile of the split's range is loaded once (cp.async, double-
+//            buffered) and scores all (<= 16) rows of the group as one mma.sync m16n8k16 A tile, as decode_attn_mq_kernel
+//            does; the CTA ropes the rows' q itself. Partial (o, m, l) of row r -> slot `split` of (r, head).
+//   z >= G : row z - G, decode_attn_cta over its suffix [P, pos] (RoPE, the append of the new row, half-warp attention), split
+//            nsplit ways. Partial -> slot nsplit + split.
+// The last CTA of a (row, head) merges its 2 * nsplit partials (nsplit for a row outside every group) in slot order and resets
+// the counter.
+// ------------------------------------------------------------------------------------------------
+constexpr size_t SH_SMEM = MQ_SMEM;
+
+struct DecodeAttnSharedParams {
+    const __nv_bfloat16* qkv;  // [B, 3*H*128], not roped
+    __nv_bfloat16* kcache;
+    __nv_bfloat16* vcache;
+    const int32_t* cur_len;    // [B]
+    const PrefixGroup* groups; // [G]
+    const int32_t* row_prefix; // [B]: P of the row's group, 0 outside every group
+    __nv_bfloat16* out;        // [B, H*128]
+    float* partial;            // [B*H][2*nsplit][128 + 2]
+    int32_t* counters;         // [B*H]
+    int G, H, Smax, nsplit;
+    float theta, scale_log2;
+};
+
+// the merge of row b's partials (slots [s0, 2 * nsplit) of (b, head)) by the CTA that completed them
+__device__ __forceinline__ void shared_merge(const DecodeAttnSharedParams& p, int b, int head, int s0) {
+    const int tid = threadIdx.x;
+    const int bh = b * p.H + head;
+    const float* pb = p.partial + (size_t)bh * 2 * p.nsplit * (DA_D + 2);
+    float m_all = -INFINITY;
+    for (int s = s0; s < 2 * p.nsplit; ++s) m_all = fmaxf(m_all, __ldcg(pb + (size_t)s * (DA_D + 2) + DA_D));
+    float l_all = 0.f, o_all = 0.f;
+#pragma unroll 4
+    for (int s = s0; s < 2 * p.nsplit; ++s) {
+        const float ms = __ldcg(pb + (size_t)s * (DA_D + 2) + DA_D);
+        const float w = (ms == -INFINITY) ? 0.f : exp2f(ms - m_all);
+        l_all += __ldcg(pb + (size_t)s * (DA_D + 2) + DA_D + 1) * w;
+        o_all += __ldcg(pb + (size_t)s * (DA_D + 2) + tid) * w;
+    }
+    p.out[(size_t)b * p.H * DA_D + head * DA_D + tid] = __float2bfloat16_rn(o_all / l_all);
+    if (tid == 0) p.counters[bh] = 0;  // self-reset for the next launch
+}
+
+__global__ void __launch_bounds__(128) decode_attn_shared_kernel(DecodeAttnSharedParams p) {
+    extern __shared__ __align__(16) uint8_t sh_smem[];
+    __shared__ int s_rows[MQ_ROWS];
+    __shared__ int s_last[MQ_ROWS];
+    const int split = blockIdx.x, head = blockIdx.y, z = blockIdx.z;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    pdl_trigger();
+    pdl_wait();  // qkv (previous GEMM) and cur_len (previous step) are upstream outputs
+    const int hd = p.H * DA_D;
+
+    if (z >= p.G) {  // ---- a row's suffix ----
+        const int b = z - p.G;
+        const int pos = p.cur_len[b], P = p.row_prefix[b];
+        float* s_q = reinterpret_cast<float*>(sh_smem);
+        float* s_knew = s_q + DA_D;
+        float* s_m = s_knew + DA_D;
+        float* s_l = s_m + 8;
+        float (*s_o)[DA_D] = reinterpret_cast<float (*)[DA_D]>(s_l + 8);
+        const int bh = b * p.H + head;
+        decode_attn_cta(p.qkv, p.kcache, p.vcache, b, head, split, p.nsplit, pos, P, p.H, p.Smax, p.theta, p.scale_log2, p.partial,
+                        2 * p.nsplit, p.nsplit, s_q, s_knew, s_m, s_l, s_o);
+        __threadfence();
+        __syncthreads();
+        if (tid == 0) {
+            const int prev = atomicAdd(&p.counters[bh], 1);
+            s_last[0] = (prev == (P > 0 ? 2 : 1) * p.nsplit - 1) ? 1 : 0;
+        }
+        __syncthreads();
+        if (s_last[0]) {
+            __threadfence();
+            shared_merge(p, b, head, P > 0 ? 0 : p.nsplit);
+        }
+        return;
+    }
+
+    // ---- a group's prefix ----
+    __nv_bfloat16* sQ = reinterpret_cast<__nv_bfloat16*>(sh_smem);  // [16][LD]
+    __nv_bfloat16* sK = sQ + MQ_ROWS * MQ_LD;                         // [2][64][LD]
+    __nv_bfloat16* sV = sK + 2 * MQ_BN * MQ_LD;                       // [2][64][LD]
+    const PrefixGroup& gr = p.groups[z];
+    const int n = gr.n_rows, P = gr.prefix_len;
+    if (tid < MQ_ROWS) s_rows[tid] = tid < n ? gr.rows[tid] : 0;
+    const int chunk = (P + p.nsplit - 1) / p.nsplit;
+    const int k_begin = min(split * chunk, P), k_end = min(k_begin + chunk, P);
+    const int n_tiles = (k_end - k_begin + MQ_BN - 1) / MQ_BN;
+    const size_t cbase = ((size_t)gr.src_slot * p.H + head) * p.Smax * DA_D;
+    const __nv_bfloat16* kg = p.kcache + cbase;
+    const __nv_bfloat16* vg = p.vcache + cbase;
+    constexpr int CH = DA_D / 8;
+    auto load_kv = [&](int tile, int buf) {
+        for (int i = tid; i < MQ_BN * CH; i += 128) {
+            const int r = i / CH, c = i % CH;
+            const int t = k_begin + tile * MQ_BN + r;
+            const bool ok = t < k_end;
+            const size_t off = (size_t)(ok ? t : 0) * DA_D + c * 8;
+            cp_async_16(sK + (buf * MQ_BN + r) * MQ_LD + c * 8, kg + off, ok);
+            cp_async_16(sV + (buf * MQ_BN + r) * MQ_LD + c * 8, vg + off, ok);
+        }
+    };
+    if (n_tiles > 0) load_kv(0, 0);
+    cp_async_commit();
+    __syncthreads();  // s_rows
+    // q of every row, roped at the row's own position exactly as decode_attn_cta ropes it (bf16 values: exact as an mma operand);
+    // rows >= n are zero
+    for (int i = tid; i < MQ_ROWS * 64; i += 128) {
+        const int r = i >> 6, e = i & 63;
+        float lo = 0.f, hi = 0.f;
+        if (r < n) {
+            const int row = s_rows[r];
+            const __nv_bfloat16* qrow = p.qkv + (size_t)row * 3 * hd + head * DA_D;
+            float cs, sn;
+            rope_cos_sin(p.cur_len[row], e, DA_D, p.theta, cs, sn);
+            const float q1 = __bfloat162float(qrow[e]), q2 = __bfloat162float(qrow[e + 64]);
+            lo = rope_apply(q1, -q2, cs, sn);
+            hi = rope_apply(q2, q1, cs, sn);
+        }
+        sQ[r * MQ_LD + e] = __float2bfloat16_rn(lo);
+        sQ[r * MQ_LD + e + 64] = __float2bfloat16_rn(hi);
+    }
+
+    uint32_t qf[DA_D / 16][4];
+    float oacc[DA_D / 8][4];
+#pragma unroll
+    for (int i = 0; i < DA_D / 8; ++i) oacc[i][0] = oacc[i][1] = oacc[i][2] = oacc[i][3] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY};
+    float l_run[2] = {0.f, 0.f};
+    const int g = lane >> 2, tq = lane & 3;  // this thread's rows: g and g + 8
+
+    for (int j = 0; j < n_tiles; ++j) {
+        if (j + 1 < n_tiles) load_kv(j + 1, (j + 1) & 1);
+        cp_async_commit();
+        cp_async_wait<1>();
+        __syncthreads();
+        if (j == 0) {
+#pragma unroll
+            for (int kk = 0; kk < DA_D / 16; ++kk)
+                ldmatrix_x4(qf[kk], sQ + ((lane & 7) + ((lane >> 3) & 1) * 8) * MQ_LD + kk * 16 + (lane >> 4) * 8);
+        }
+        const __nv_bfloat16* tK = sK + ((j & 1) * MQ_BN + warp * 16) * MQ_LD;
+        const __nv_bfloat16* tV = sV + ((j & 1) * MQ_BN + warp * 16) * MQ_LD;
+
+        float s[2][4];
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt) s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
+#pragma unroll
+        for (int kk = 0; kk < DA_D / 16; ++kk) {
+            uint32_t bfr[4];
+            ldmatrix_x4(bfr, tK + ((lane & 7) + (lane >> 4) * 8) * MQ_LD + kk * 16 + ((lane >> 3) & 1) * 8);
+            mma_bf16_16816(s[0], qf[kk], bfr[0], bfr[1]);
+            mma_bf16_16816(s[1], qf[kk], bfr[2], bfr[3]);
+        }
+
+        // every row's position is >= P: the only limit is the end of the split's range
+        const int key0 = k_begin + j * MQ_BN + warp * 16;
+        float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int key = key0 + nt * 8 + tq * 2 + (e & 1);
+                const float val = key < k_end ? s[nt][e] * p.scale_log2 : -INFINITY;
+                s[nt][e] = val;
+                mx[e >> 1] = fmaxf(mx[e >> 1], val);
+            }
+        }
+        float corr[2], m_use[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+            mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+            const float m_new = fmaxf(m_run[h], mx[h]);
+            m_use[h] = (m_new == -INFINITY) ? 0.f : m_new;
+            corr[h] = exp2f(m_run[h] - m_use[h]);
+            m_run[h] = m_new;
+            l_run[h] *= corr[h];
+        }
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float pv = exp2f(s[nt][e] - m_use[e >> 1]);
+                s[nt][e] = pv;
+                l_run[e >> 1] += pv;
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < DA_D / 8; ++i) {
+            oacc[i][0] *= corr[0]; oacc[i][1] *= corr[0];
+            oacc[i][2] *= corr[1]; oacc[i][3] *= corr[1];
+        }
+        // O += P V with P = hi + lo bf16 operands
+        uint32_t pa[4], pl[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const float x0 = s[i >> 1][(i & 1) * 2], x1 = s[i >> 1][(i & 1) * 2 + 1];
+            pa[i] = pack_bf16(x0, x1);
+            pl[i] = pack_bf16(x0 - bf16_lo(pa[i]), x1 - bf16_hi(pa[i]));
+        }
+#pragma unroll
+        for (int dp = 0; dp < DA_D / 16; ++dp) {
+            uint32_t bfr[4];
+            ldmatrix_x4_trans(bfr, tV + ((lane & 7) + ((lane >> 3) & 1) * 8) * MQ_LD + dp * 16 + (lane >> 4) * 8);
+            mma_bf16_16816(oacc[2 * dp], pa, bfr[0], bfr[1]);
+            mma_bf16_16816(oacc[2 * dp + 1], pa, bfr[2], bfr[3]);
+            mma_bf16_16816(oacc[2 * dp], pl, bfr[0], bfr[1]);
+            mma_bf16_16816(oacc[2 * dp + 1], pl, bfr[2], bfr[3]);
+        }
+        __syncthreads();  // buffer (j & 1) is refilled at iteration j + 1
+    }
+    cp_async_wait<0>();
+    __syncthreads();
+
+    // ---- merge the four warps, one partial per row of the group ----
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
+        l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
+    }
+    float* s_o = reinterpret_cast<float*>(sK);   // [4][16][128]
+    float* s_ml = reinterpret_cast<float*>(sV);  // [4][16][2]
+#pragma unroll
+    for (int i = 0; i < DA_D / 8; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+            s_o[(warp * MQ_ROWS + g + (e >> 1) * 8) * DA_D + i * 8 + tq * 2 + (e & 1)] = oacc[i][e];
+    if (tq == 0)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            s_ml[(warp * MQ_ROWS + g + h * 8) * 2] = m_run[h];
+            s_ml[(warp * MQ_ROWS + g + h * 8) * 2 + 1] = l_run[h];
+        }
+    __syncthreads();
+    for (int r = 0; r < n; ++r) {  // thread tid owns output column tid
+        float m_cta = -INFINITY;
+#pragma unroll
+        for (int w = 0; w < 4; ++w) m_cta = fmaxf(m_cta, s_ml[(w * MQ_ROWS + r) * 2]);
+        float l_cta = 0.f, o_cta = 0.f;
+#pragma unroll
+        for (int w = 0; w < 4; ++w) {
+            const float mw = s_ml[(w * MQ_ROWS + r) * 2];
+            const float wt = (mw == -INFINITY) ? 0.f : exp2f(mw - m_cta);
+            l_cta += s_ml[(w * MQ_ROWS + r) * 2 + 1] * wt;
+            o_cta += s_o[(w * MQ_ROWS + r) * DA_D + tid] * wt;
+        }
+        float* part = p.partial + (((size_t)s_rows[r] * p.H + head) * 2 * p.nsplit + split) * (DA_D + 2);
+        part[tid] = o_cta;
+        if (tid == 0) { part[DA_D] = m_cta; part[DA_D + 1] = l_cta; }
+    }
+
+    // ---- the last CTA of a (row, head) merges that row ----
+    __threadfence();
+    __syncthreads();
+    if (tid < n) {
+        const int prev = atomicAdd(&p.counters[s_rows[tid] * p.H + head], 1);
+        s_last[tid] = (prev == 2 * p.nsplit - 1) ? 1 : 0;
+    }
+    __syncthreads();
+    for (int r = 0; r < n; ++r) {
+        if (!s_last[r]) continue;  // CTA-uniform
+        __threadfence();
+        shared_merge(p, s_rows[r], head, 0);
     }
 }
 
@@ -948,6 +1235,51 @@ int decode_attn_mq_bf16(const DecodeAttnArgs& a, cudaStream_t stream) {
     p.R = a.R; p.H = a.H; p.Smax = a.Smax; p.nsplit = a.nsplit;
     p.scale_log2 = a.scale * 1.4426950408889634f;
     B2_CUDA_CHECK(launch_pdl(decode_attn_mq_kernel, dim3(a.nsplit, a.H, a.B), dim3(128), MQ_SMEM, stream, p));
+    B2_LAUNCH_CHECK();
+    return 0;
+}
+
+// resident CTAs of decode_attn_shared_kernel per SM (shared-memory-limited like decode_attn_mq_kernel), for the split heuristic
+int decode_attn_shared_ctas_per_sm() {
+    static int occ = 0;
+    if (occ == 0) {
+        int n = 0;
+        if (cudaFuncSetAttribute(decode_attn_shared_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SH_SMEM) != cudaSuccess ||
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, decode_attn_shared_kernel, 128, SH_SMEM) != cudaSuccess || n < 1) {
+            cudaGetLastError();
+            n = 3;
+        }
+        occ = n;
+    }
+    return occ;
+}
+
+size_t decode_attn_shared_scratch_bytes(int B, int H, int nsplit) {
+    return (size_t)B * H * 2 * nsplit * (DA_D + 2) * sizeof(float) + (size_t)B * H * sizeof(int32_t);
+}
+
+int decode_attn_shared_bf16(const DecodeAttnArgs& a, const PrefixGroup* groups, const int32_t* row_prefix, int G,
+                            cudaStream_t stream) {
+    B2_CHECK_ARG(a.D == DA_D, "decode_attn_shared: head_dim must be 128 (got %d)", a.D);
+    B2_CHECK_ARG(a.nsplit >= 1 && a.B > 0 && a.H > 0 && G >= 0 && G <= a.B, "decode_attn_shared: bad launch shape");
+    B2_CHECK_ARG(G == 0 || (groups != nullptr && row_prefix != nullptr), "decode_attn_shared: null group table");
+    B2_CHECK_ARG(((reinterpret_cast<uintptr_t>(a.qkv) | reinterpret_cast<uintptr_t>(a.kcache) |
+                   reinterpret_cast<uintptr_t>(a.vcache)) & 15) == 0, "decode_attn_shared: buffers must be 16-byte aligned");
+    decode_attn_shared_ctas_per_sm();  // sets the dynamic shared-memory attribute
+    DecodeAttnSharedParams p;
+    p.qkv = reinterpret_cast<const __nv_bfloat16*>(a.qkv);
+    p.kcache = reinterpret_cast<__nv_bfloat16*>(a.kcache);
+    p.vcache = reinterpret_cast<__nv_bfloat16*>(a.vcache);
+    p.cur_len = a.cur_len;
+    p.groups = groups;
+    p.row_prefix = row_prefix;
+    p.out = reinterpret_cast<__nv_bfloat16*>(a.out);
+    p.partial = a.partial;
+    p.counters = a.counters;
+    p.G = G; p.H = a.H; p.Smax = a.Smax; p.nsplit = a.nsplit;
+    p.theta = a.theta;
+    p.scale_log2 = a.scale * 1.4426950408889634f;
+    B2_CUDA_CHECK(launch_pdl(decode_attn_shared_kernel, dim3(a.nsplit, a.H, G + a.B), dim3(128), SH_SMEM, stream, p));
     B2_LAUNCH_CHECK();
     return 0;
 }

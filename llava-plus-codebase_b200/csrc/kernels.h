@@ -170,6 +170,20 @@ int decode_attn_bf16(const DecodeAttnArgs& a, cudaStream_t stream);
 int decode_attn_mq_ctas_per_sm();
 size_t decode_attn_mq_scratch_bytes(int B, int H, int nsplit);  // partial then counters
 int decode_attn_mq_bf16(const DecodeAttnArgs& a, cudaStream_t stream);
+// shared-prefix decode (the forked samples of one prompt): decode_attn_bf16's result for every row, with keys [0, prefix_len) of
+// a group's rows read once per group from its source slot. Same layout as b2_prefix_group (include/b2llava.h).
+constexpr int kPrefixGroupRows = 16;
+struct PrefixGroup {
+    int32_t src_slot, prefix_len, n_rows;
+    int32_t rows[kPrefixGroupRows];
+};
+// groups: device [G]; row_prefix: device [B], the prefix_len of the row's group (0 outside every group). G <= B, every row in
+// at most one group, 1 <= prefix_len <= cur_len of the source and of every member. partial: [B*H*2*nsplit*(D+2)] fp32, then the
+// counters [B*H] (decode_attn_shared_scratch_bytes)
+int decode_attn_shared_ctas_per_sm();
+size_t decode_attn_shared_scratch_bytes(int B, int H, int nsplit);  // partial then counters
+int decode_attn_shared_bf16(const DecodeAttnArgs& a, const PrefixGroup* groups, const int32_t* row_prefix, int G,
+                            cudaStream_t stream);
 // the same step over an e4m3 cache (rows of 128 bytes + one fp32 scale per row); Smax % 4 == 0
 int decode_attn_e4m3_ctas_per_sm();
 int decode_attn_e4m3(const DecodeAttnArgs& a, cudaStream_t stream);

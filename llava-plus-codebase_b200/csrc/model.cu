@@ -205,6 +205,11 @@ struct b2_kv {
     std::array<cudaGraphExec_t, kSpecMaxRows + 1> spec_graph{};
     std::array<int, kSpecMaxRows + 1> spec_launches{};
     std::array<char, kSpecMaxRows + 1> spec_warm{};
+    // shared-prefix decode (b2_stream_begin_groups; allocated by its first call, not counted by b2_kv_bytes): the group table
+    // PrefixGroup[max_batch] then row_prefix int32 [max_batch], and decode_attn_shared's partials and counters. share_G > 0 while
+    // a generation runs with the table armed; the multi-kernel step over a bf16 cache then reads it.
+    DevBuf share_tab, share_attn;
+    int share_G = 0;
     bool counted = false;  // included in m->kv_live
     bool e4m3() const { return dtype == B2_KV_E4M3; }
     size_t elem_bytes() const { return e4m3() ? 1 : 2; }
@@ -628,11 +633,16 @@ int encode_chunk(b2_model* m, const void* pixels, int n, void* out, cudaStream_t
     return 0;
 }
 
+// the counters at the front of kv->share_attn (every row of the cache, 256-byte aligned partials behind them)
+size_t share_counter_bytes(const b2_kv* kv) { return ((size_t)kv->max_batch * kv->m->d.heads * sizeof(int32_t) + 255) / 256 * 256; }
+
 // one decode step on kv-owned buffers: tok -> logits (m->logits) -> argmax -> tok, out_tokens[step], len += 1
 int decode_step_launch(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     const b2_model_desc& d = m->d;
     const int h = d.hidden, I = d.inter, H = d.heads, V = d.vocab;
-    const int nsplit = decode_nsplit(B, H, kv->max_seq, kv->e4m3() ? decode_attn_e4m3_ctas_per_sm() : decode_attn_ctas_per_sm());
+    const bool shared = kv->share_G > 0 && !kv->e4m3();
+    const int nsplit = decode_nsplit(B, H, kv->max_seq, kv->e4m3() ? decode_attn_e4m3_ctas_per_sm()
+                                                        : shared ? decode_attn_shared_ctas_per_sm() : decode_attn_ctas_per_sm());
     const DecodePlan plan = decode_plan(m, kv, B);
     const DecodePath p = plan.layer;
     B2_TRY(embed_tokens(kv->tok.as<int32_t>(), m->embed.p, m->x.p, B, h, V, m->err_dev, st));
@@ -656,6 +666,12 @@ int decode_step_launch(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
             da.kscale = kv->kscale.as<float>() + (size_t)l * kv->layer_rows();
             da.vscale = kv->vscale.as<float>() + (size_t)l * kv->layer_rows();
             B2_TRY(decode_attn_e4m3(da, st));
+        } else if (shared) {
+            const PrefixGroup* groups = kv->share_tab.as<PrefixGroup>();
+            // counters first, at a place that does not move with B and nsplit: they stay zero between launches
+            da.counters = kv->share_attn.as<int32_t>();
+            da.partial = reinterpret_cast<float*>(kv->share_attn.as<char>() + share_counter_bytes(kv));
+            B2_TRY(decode_attn_shared_bf16(da, groups, reinterpret_cast<const int32_t*>(groups + kv->max_batch), kv->share_G, st));
         } else {
             B2_TRY(decode_attn_bf16(da, st));
         }
@@ -767,6 +783,14 @@ int decode_step_mega(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     return 0;
 }
 
+// the shared-prefix group table (b2_stream_begin_groups) := G groups armed, 0 disarmed. A change drops the captured decode graph
+// and makes the next step eager, as a first step at a batch size is (it sets the shared kernel's function attributes).
+static void share_arm(b2_kv* kv, int G) {
+    if (kv->share_G == G) return;
+    if (kv->graph) { cudaGraphExecDestroy(kv->graph); kv->graph = nullptr; kv->graph_B = 0; }
+    kv->warm_B = 0;
+    kv->share_G = G;
+}
 int decode_step_run(b2_model* m, b2_kv* kv, int B, cudaStream_t st) {
     // B <= 8: one persistent cooperative launch per token (no graph needed: launches queue asynchronously)
     if (use_mega(m, kv, B)) return decode_step_mega(m, kv, B, st);
@@ -897,7 +921,7 @@ int b2_init(int device) {
 }
 
 const char* b2_last_error(void) { return g_err; }
-int b2_version(void) { return 10; }
+int b2_version(void) { return 11; }
 unsigned long long b2_launch_count(void) { return g_launch_count; }
 
 int b2_model_create(const b2_model_desc* desc, b2_model** out) {
@@ -1333,6 +1357,7 @@ int b2_kv_reset(b2_kv* kv) {
     // decode call, both on the CALLER's stream; a cudaMemset here would run on the legacy stream, unordered against work
     // still in flight on a non-blocking caller stream (e.g. two forward() calls issued back to back).
     kv->len_host.assign(kv->max_batch, 0);
+    share_arm(kv, 0);  // the table names prefix lengths of the contents just dropped
     {   // measurement knob: drop the captured decode graph so that the next run starts with an eager step + a new capture
         const char* e = getenv("B2_KV_RESET_GRAPH");
         if (e != nullptr && e[0] == '1') {
@@ -1611,8 +1636,9 @@ static int set_sampling(b2_kv* kv, const SampleState& v, bool force, cudaStream_
     return 0;
 }
 // every slot selects from its raw logits again (a no-op on a cache whose processors are off); beam processing is disarmed
-// unless keep_beam (the step of a processed beam search itself)
+// unless keep_beam (the step of a processed beam search itself), and so is the shared-prefix group table
 static int proc_all_off(b2_kv* kv, cudaStream_t st, bool keep_beam = false) {
+    share_arm(kv, 0);
     if (!keep_beam) kv->beam_proc_on = false;
     if (!kv->any_proc()) return 0;
     B2_CUDA_CHECK(cudaMemsetAsync(kv->proc_rows.p, 0, kv->proc_rows.bytes, st));
@@ -2078,12 +2104,40 @@ int b2_stream_set_outputs(b2_kv* kv, float* scores, float* logits, int cap_steps
     return 0;
 }
 
+// the shared-prefix state of a cache, allocated by the first armed generation: the table, and the counters of max_batch rows
+// (zeroed on `st`; they self-reset after every launch) followed by partials for the largest split decode_nsplit gives (16)
+static int share_alloc(b2_model* m, b2_kv* kv, cudaStream_t st) {
+    if (kv->share_tab.p != nullptr) return 0;
+    const size_t attn = share_counter_bytes(kv) + decode_attn_shared_scratch_bytes(kv->max_batch, m->d.heads, 16);
+    int r = kv->share_tab.alloc((size_t)kv->max_batch * (sizeof(PrefixGroup) + sizeof(int32_t)));
+    if (r == 0) r = kv->share_attn.alloc(attn);
+    if (r == 0 && cudaMemsetAsync(kv->share_attn.p, 0, attn, st) != cudaSuccess) {
+        set_error("b2_stream_begin_groups: %s", cudaGetErrorString(cudaGetLastError()));
+        r = -2;
+    }
+    if (r != 0) { kv->share_tab.free(); kv->share_attn.free(); }
+    return r;
+}
+static int stream_begin(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sp, const b2_logits_proc* proc,
+                        const b2_prefix_group* groups, int G, void* stream);
+
 int b2_stream_begin(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sp, void* stream) {
     return b2_stream_begin_ex(m, kv, logits, B, sp, nullptr, stream);
 }
 
 int b2_stream_begin_ex(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sp, const b2_logits_proc* proc,
                        void* stream) {
+    return stream_begin(m, kv, logits, B, sp, proc, nullptr, 0, stream);
+}
+
+int b2_stream_begin_groups(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sp, const b2_logits_proc* proc,
+                           const b2_prefix_group* groups, int G, void* stream) {
+    B2_CHECK_ARG(G >= 1 && groups != nullptr, "b2_stream_begin_groups: G=%d groups (at least one)", G);
+    return stream_begin(m, kv, logits, B, sp, proc, groups, G, stream);
+}
+
+static int stream_begin(b2_model* m, b2_kv* kv, const float* logits, int B, const b2_sampling* sp, const b2_logits_proc* proc,
+                        const b2_prefix_group* groups, int G, void* stream) {
     B2_CHECK_ARG(m && kv && logits && kv->m == m, "b2_stream_begin: bad handle");
     // the rows armed by b2_stream_set_outputs belong to this call, whether or not it begins a generation
     float *out_scores, *out_logits;
@@ -2111,6 +2165,34 @@ int b2_stream_begin_ex(b2_model* m, b2_kv* kv, const float* logits, int B, const
         B2_CHECK_ARG(kv->len_host[b] >= 1, "b2_stream_begin: sample %d has an empty cache (prefill first)", b);
     std::vector<ProcRow> pr(B);
     for (int b = 0; b < B; ++b) B2_TRY(proc_row_of(proc ? proc + b : nullptr, kv->max_seq + 1, &pr[b], "b2_stream_begin_ex"));
+    // the group table: checked against the cache before anything is queued
+    std::vector<PrefixGroup> tab(G);
+    std::vector<int32_t> row_prefix(kv->max_batch, 0);
+    if (G > 0) {
+        B2_CHECK_ARG(G <= B, "b2_stream_begin_groups: G=%d groups for %d rows", G, B);
+        std::vector<char> seen(B, 0);
+        for (int g = 0; g < G; ++g) {
+            const b2_prefix_group& x = groups[g];
+            B2_CHECK_ARG(x.n_rows >= 1 && x.n_rows <= kPrefixGroupRows, "b2_stream_begin_groups: group %d has %d rows (1..%d)", g,
+                         x.n_rows, kPrefixGroupRows);
+            B2_CHECK_ARG(x.src_slot >= 0 && x.src_slot < B, "b2_stream_begin_groups: group %d source slot %d outside [0, %d)", g,
+                         x.src_slot, B);
+            B2_CHECK_ARG(x.prefix_len >= 1 && x.prefix_len <= kv->len_host[x.src_slot],
+                         "b2_stream_begin_groups: group %d prefix_len %d outside [1, %d] (the length of slot %d)", g, x.prefix_len,
+                         kv->len_host[x.src_slot], x.src_slot);
+            tab[g].src_slot = x.src_slot; tab[g].prefix_len = x.prefix_len; tab[g].n_rows = x.n_rows;
+            for (int r = 0; r < kPrefixGroupRows; ++r) tab[g].rows[r] = r < x.n_rows ? x.rows[r] : 0;
+            for (int r = 0; r < x.n_rows; ++r) {
+                const int row = x.rows[r];
+                B2_CHECK_ARG(row >= 0 && row < B, "b2_stream_begin_groups: group %d row %d outside [0, %d)", g, row, B);
+                B2_CHECK_ARG(!seen[row], "b2_stream_begin_groups: row %d belongs to two groups", row);
+                B2_CHECK_ARG(x.prefix_len <= kv->len_host[row], "b2_stream_begin_groups: group %d prefix_len %d exceeds the length %d "
+                             "of its row %d", g, x.prefix_len, kv->len_host[row], row);
+                seen[row] = 1;
+                row_prefix[row] = x.prefix_len;
+            }
+        }
+    }
     kv->epoch += 1;
     v.tag = 1 + kv->epoch % 2047;
     kv->spec_R = 0;
@@ -2125,6 +2207,14 @@ int b2_stream_begin_ex(b2_model* m, b2_kv* kv, const float* logits, int B, const
                           kv->step_counter.as<int32_t>(), kv->len_dev.as<int32_t>(), kv->ring_dev, kv->ring_cap, SP_SELECT, 0,
                           proc_state(kv), nullptr, st));
     kv->stream_B = B; kv->stream_tag = v.tag; kv->stream_scheduled = 1;
+    if (G > 0) {
+        B2_TRY(share_alloc(m, kv, st));
+        B2_CUDA_CHECK(cudaMemcpyAsync(kv->share_tab.p, tab.data(), (size_t)G * sizeof(PrefixGroup), cudaMemcpyHostToDevice, st));
+        B2_CUDA_CHECK(cudaMemcpyAsync(kv->share_tab.as<PrefixGroup>() + kv->max_batch, row_prefix.data(),
+                                      (size_t)kv->max_batch * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+        B2_CUDA_CHECK(cudaStreamSynchronize(st));  // pageable host sources
+        share_arm(kv, G);
+    }
     return ws_leave(m, st);
 }
 
@@ -2611,6 +2701,51 @@ int b2_op_prompt_lookup(const int32_t* hist, int len, int num_tokens, int max_ng
     tmp.free();
     if (r != 0) return r;
     B2_CUDA_CHECK(e);
+    return 0;
+}
+
+int64_t b2_op_decode_attn_shared_scratch_bytes(int B, int H, int nsplit) {
+    if (B < 1 || H < 1 || nsplit < 1) return -1;
+    return (int64_t)(decode_attn_shared_scratch_bytes(B, H, nsplit) + (size_t)B * (sizeof(PrefixGroup) + sizeof(int32_t)));
+}
+
+int b2_op_decode_attn_shared_nsplit(int B, int H, int Smax) {
+    B2_CHECK_ARG(B >= 1 && H >= 1 && Smax >= 1, "b2_op_decode_attn_shared_nsplit: bad shape");
+    return decode_nsplit(B, H, Smax, decode_attn_shared_ctas_per_sm());
+}
+
+int b2_op_decode_attn_shared(const void* qkv, void* kcache, void* vcache, const int32_t* cur_len, const b2_prefix_group* groups_host,
+                             int G, void* out, void* scratch, int B, int H, int Smax, int nsplit, float theta, float scale,
+                             void* stream) {
+    B2_CHECK_ARG(qkv && kcache && vcache && cur_len && out && scratch && (G == 0 || groups_host), "b2_op_decode_attn_shared: null argument");
+    B2_CHECK_ARG(B >= 1 && H >= 1 && nsplit >= 1 && Smax >= 1 && G >= 0 && G <= B, "b2_op_decode_attn_shared: bad shape");
+    std::vector<PrefixGroup> tab(G);
+    std::vector<int32_t> row_prefix(B, 0);
+    for (int g = 0; g < G; ++g) {
+        const b2_prefix_group& x = groups_host[g];
+        B2_CHECK_ARG(x.n_rows >= 1 && x.n_rows <= kPrefixGroupRows && x.src_slot >= 0 && x.src_slot < B && x.prefix_len >= 1 &&
+                     x.prefix_len <= Smax, "b2_op_decode_attn_shared: bad group %d", g);
+        tab[g].src_slot = x.src_slot; tab[g].prefix_len = x.prefix_len; tab[g].n_rows = x.n_rows;
+        for (int r = 0; r < kPrefixGroupRows; ++r) tab[g].rows[r] = r < x.n_rows ? x.rows[r] : 0;
+        for (int r = 0; r < x.n_rows; ++r) {
+            B2_CHECK_ARG(x.rows[r] >= 0 && x.rows[r] < B && row_prefix[x.rows[r]] == 0, "b2_op_decode_attn_shared: group %d row %d", g,
+                         x.rows[r]);
+            row_prefix[x.rows[r]] = x.prefix_len;
+        }
+    }
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const size_t attn = decode_attn_shared_scratch_bytes(B, H, nsplit);
+    PrefixGroup* dtab = reinterpret_cast<PrefixGroup*>(reinterpret_cast<char*>(scratch) + attn);
+    int32_t* dprefix = reinterpret_cast<int32_t*>(dtab + B);
+    if (G > 0) B2_CUDA_CHECK(cudaMemcpyAsync(dtab, tab.data(), (size_t)G * sizeof(PrefixGroup), cudaMemcpyHostToDevice, st));
+    B2_CUDA_CHECK(cudaMemcpyAsync(dprefix, row_prefix.data(), (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    DecodeAttnArgs da;
+    da.qkv = qkv; da.kcache = kcache; da.vcache = vcache; da.cur_len = cur_len; da.out = out;
+    da.partial = reinterpret_cast<float*>(scratch);
+    da.counters = reinterpret_cast<int32_t*>(reinterpret_cast<char*>(scratch) + attn - (size_t)B * H * sizeof(int32_t));
+    da.B = B; da.H = H; da.D = 128; da.Smax = Smax; da.nsplit = nsplit; da.theta = theta; da.scale = scale;
+    B2_TRY(decode_attn_shared_bf16(da, dtab, dprefix, G, st));
+    B2_CUDA_CHECK(cudaStreamSynchronize(st));  // pageable host sources
     return 0;
 }
 

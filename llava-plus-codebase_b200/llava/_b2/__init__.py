@@ -82,6 +82,23 @@ class LogitsProc(_c.Structure):
 MAX_PROC_EOS = 8
 
 
+class PrefixGroup(_c.Structure):
+    """b2_prefix_group (include/b2llava.h): rows of one batch that read keys [0, prefix_len) from slot src_slot."""
+    _fields_ = [("src_slot", _c.c_int32), ("prefix_len", _c.c_int32), ("n_rows", _c.c_int32), ("rows", _c.c_int32 * 16)]
+
+
+def _group_array(groups):
+    """ctypes array of PrefixGroup from (src_slot, prefix_len, rows) triples."""
+    arr = (PrefixGroup * len(groups))()
+    for i, (src, plen, rows) in enumerate(groups):
+        if not 1 <= len(rows) <= 16:
+            raise ValueError(f"a prefix group holds 1..16 rows, got {len(rows)}")
+        arr[i].src_slot, arr[i].prefix_len, arr[i].n_rows = int(src), int(plen), len(rows)
+        for j, r in enumerate(rows):
+            arr[i].rows[j] = int(r)
+    return arr
+
+
 class PromptLookup(_c.Structure):
     """b2_prompt_lookup (include/b2llava.h): prompt-lookup speculative decoding of one sample; `prompt_ids` is a device int64
     pointer."""
@@ -172,6 +189,8 @@ SIGNATURES = {
     "b2_async_error": (_i32, [_vp, _c.POINTER(_c.c_int)]),
     "b2_stream_begin": (_i32, [_vp, _vp, _vp, _i32, _c.POINTER(Sampling), _vp]),
     "b2_stream_begin_ex": (_i32, [_vp, _vp, _vp, _i32, _c.POINTER(Sampling), _c.POINTER(LogitsProc), _vp]),
+    "b2_stream_begin_groups": (_i32, [_vp, _vp, _vp, _i32, _c.POINTER(Sampling), _c.POINTER(LogitsProc), _c.POINTER(PrefixGroup), _i32,
+                                      _vp]),
     "b2_stream_enqueue": (_i32, [_vp, _vp, _i32, _vp]),
     "b2_stream_wait": (_i32, [_vp, _i32, _c.POINTER(_c.c_int32), _i32]),
     "b2_stream_set_outputs": (_i32, [_vp, _vp, _vp, _i32]),
@@ -226,6 +245,10 @@ SIGNATURES = {
     "b2_op_decode_attn_mq": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _vp]),
     "b2_op_decode_attn_mq_scratch_bytes": (_i64, [_i32, _i32, _i32]),
     "b2_op_decode_attn_mq_nsplit": (_i32, [_i32, _i32]),
+    "b2_op_decode_attn_shared": (_i32, [_vp, _vp, _vp, _vp, _c.POINTER(PrefixGroup), _i32, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _f32,
+                                        _vp]),
+    "b2_op_decode_attn_shared_scratch_bytes": (_i64, [_i32, _i32, _i32]),
+    "b2_op_decode_attn_shared_nsplit": (_i32, [_i32, _i32, _i32]),
     "b2_op_prompt_lookup": (_i32, [_vp, _i32, _i32, _i32, _i32, _c.POINTER(_c.c_int32), _i32, _i32, _vp, _vp, _vp]),
     "b2_op_kv_quantize_e4m3": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
     "b2_op_kv_quantize_e4m3_at": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
@@ -519,12 +542,15 @@ class Engine:
         return out
 
     # -- streaming decode (device runs ahead, host reads tokens from mapped pinned memory) ---------------
-    def stream_begin(self, kv, logits, sampling=None, procs=None, out_scores=None, out_logits=None):
+    def stream_begin(self, kv, logits, sampling=None, procs=None, out_scores=None, out_logits=None, groups=None, share_prefix=True):
         """Token 0 is chosen from the prefill logits [B, vocab] on the device and published as ring index 0. `procs`: one
         LogitsProc (or None) per row; rows with processors keep their history on the device for the whole generation.
         `out_scores` / `out_logits` (device fp32 [steps, B, vocab], or None): the step that publishes token t writes its score
         row (what selection read: processed, and when sampling divided by T and filtered) and its raw logits row to index t
-        (b2_stream_set_outputs). Keep them alive until the generation's steps have run."""
+        (b2_stream_set_outputs). Keep them alive until the generation's steps have run. `groups` ((src_slot, prefix_len, rows)
+        triples, see llava/_b2/fork.py): rows that hold copies of one prompt's cache rows, whose decode attention then reads the
+        prompt once per group (b2_stream_begin_groups); share_prefix=False runs the same generation with every row reading its
+        own copy."""
         logits = logits.contiguous()
         sp = sampling if sampling is not None else make_sampling()
         B = int(logits.shape[0])
@@ -538,7 +564,11 @@ class Engine:
         with torch.cuda.device(self.index):
             # always armed (NULLs included): a begin never inherits buffers a failed call left behind
             check(self.lib.b2_stream_set_outputs(kv.handle, ptr(out_scores), ptr(out_logits), cap), "b2_stream_set_outputs")
-            if arr is None:
+            if groups and share_prefix:
+                g = _group_array(groups)
+                check(self.lib.b2_stream_begin_groups(self.handle, kv.handle, ptr(logits), B, ctypes.byref(sp), arr, g, len(groups),
+                                                      stream_ptr()), "b2_stream_begin_groups")
+            elif arr is None:
                 check(self.lib.b2_stream_begin(self.handle, kv.handle, ptr(logits), B, ctypes.byref(sp), stream_ptr()),
                       "b2_stream_begin")
             else:

@@ -29,6 +29,7 @@ from ..._b2 import (Engine, KVCache, LOGITS_ALL, LOGITS_LAST, ERR_SPLICE_SLOTS, 
                      make_prompt_lookup,
                     make_sampling, make_beam_sampling)
 from ..._b2 import prefix as _prefix
+from ..._b2.fork import ForkPlan
 from ...constants import IMAGE_TOKEN_INDEX
 from ..llava_arch import build_source_index
 
@@ -511,7 +512,14 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         ids, would give; every position up to and including its eos is. `past_key_values`, `attentions` and `hidden_states`
         are None. Stopping criteria still receive scores=None: handing them the live device rows would need a synchronisation
         per token. Without return_dict_in_generate the id tensor is returned and output_scores / output_logits are ignored,
-        as in HF."""
+        as in HF.
+
+        num_return_sequences=n with do_sample (and num_beams=1) returns B * n rows in HF's order (the n samples of prompt b are
+        rows b * n .. b * n + n - 1). Each prompt and its image are encoded and prefilled once; the prompt's cache rows are then
+        copied into the slots of its other samples, and the decode attention reads each prompt once for all of its samples. Token
+        0 of every sample is drawn from its prompt's prefill logits with the sample's own Philox key, so a seeded run equals HF's
+        (which repeats the inputs n times) in distribution, not in ids. Processors, score rows, stopping criteria, eos / pad and
+        the streamer see the B * n rows."""
         if inputs is None:
             inputs = input_ids
         if inputs is None:
@@ -528,7 +536,8 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 raise NotImplementedError("beam search is not used on the LLaVA path (num_beams=1 everywhere)")
             beam_args = self._beam_arguments(num_beams, do_sample, temperature, top_p, top_k, streamer, kwargs)
         prompt = inputs if inputs.dim() == 2 else inputs.unsqueeze(0)
-        lookup_args = self._prompt_lookup_arguments(kwargs, prompt.shape[0], num_beams, bool(proc_args))
+        n_ret = 1 if num_beams != 1 else _num_return_arguments(self.config, kwargs, prompt.shape[0], do_sample, images)
+        lookup_args = self._prompt_lookup_arguments(kwargs, prompt.shape[0] * n_ret, num_beams, bool(proc_args))
         if want and (want["scores"] or want["logits"]):
             what = "output_scores / output_logits with return_dict_in_generate"
             if lookup_args:
@@ -583,7 +592,7 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         began_lookup = [False]
         prof = _StageTimer() if os.environ.get("B2_PROFILE_GENERATE") else None
 
-        batcher = self._get_batcher(engine) if B == 1 else None
+        batcher = self._get_batcher(engine) if B == 1 and n_ret == 1 else None
         if batcher is not None:
             # continuous batching: this thread splices its prompt and runs its own host loop (streamer, eos, criteria); the
             # decode steps are shared with every other generate() in flight (llava/_b2/batching.py)
@@ -613,12 +622,19 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             out = torch.cat([prompt, new_tokens.to(device=prompt.device, dtype=prompt.dtype)], dim=1)
             return out if not want else _decoder_output(out, None, None)
 
+        # num_return_sequences: the B * n rows in HF's order (repeat_interleave) for the result, the streamer and the criteria;
+        # on the device prompt b is prefilled once and forked into the slots of its other samples (llava/_b2/fork.py)
+        rows_out = prompt if n_ret == 1 else prompt.repeat_interleave(n_ret, dim=0)
+        N = B * n_ret
+        fork = None
+        if n_ret > 1 and procs is not None:
+            procs = [p for p in procs for _ in range(n_ret)]  # HF row order; reordered to slots once the fork is planned
         # score / logits rows of every step the generation may take, written by the device (b2_stream_set_outputs)
-        rows = {k: (torch.empty(max_new_tokens, B, engine.vocab, dtype=torch.float32, device=engine.device) if want and want[k] else None)
+        rows = {k: (torch.empty(max_new_tokens, N, engine.vocab, dtype=torch.float32, device=engine.device) if want and want[k] else None)
                 for k in ("scores", "logits")}
         # conversation prefix reuse (opt-in, batch 1): the part of the prompt a released cache already holds is not prefilled again
         plan = None
-        if B == 1 and self._prefix_cache_on() and (attention_mask is None or bool(attention_mask.bool().all())):
+        if B == 1 and n_ret == 1 and self._prefix_cache_on() and (attention_mask is None or bool(attention_mask.bool().all())):
             plan = self._prefix_plan(prompt, images)
         reuse, released_ev = 0, None
         if plan is not None:
@@ -629,18 +645,30 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
         try:
             # ---- prefill: splice + decoder, last-position logits only; token 0 is chosen on the device ----
             def prefill(force_host):
+                nonlocal fork
                 embeds, lens, speculative = self._prompt_embeds(engine, prompt, attention_mask, images, force_host)
                 if prof: prof.mark("encode_images+splice")
-                self._check_limits(engine, B, max(lens) + max_new_tokens)
+                self._check_limits(engine, N, max(lens) + max_new_tokens)
                 kv.reset()
                 logits = engine.prefill(kv, embeds, lens, LOGITS_LAST)
                 lk = lookup(lens[0]) if lookup is not None else None
                 began_lookup[0] = lk is not None
                 if lk is not None:
                     engine.stream_begin_lookup(kv, logits, sampling, lk)
+                elif n_ret > 1:
+                    fork = ForkPlan(lens, n_ret)
+                    engine.kv_copy_slots(kv, *fork.copies())
+                    # token 0 of every sample from its prompt's prefill row, drawn with the sample's own row key
+                    logits = logits.index_select(0, torch.tensor(fork.prompt_of_slot, device=logits.device))
+                    slot_procs = None
+                    if procs is not None:
+                        slot_procs = [None] * N
+                        for r, s in enumerate(fork.slot_of_row):
+                            slot_procs[s] = procs[r]
+                    engine.stream_begin(kv, logits, sampling, slot_procs, rows["scores"], rows["logits"], groups=fork.groups())
                 else:
                     engine.stream_begin(kv, logits, sampling, procs, rows["scores"], rows["logits"])
-                engine.stream_wait(kv, 0, B)          # first sync of this call: every input check has run by now
+                engine.stream_wait(kv, 0, N)          # first sync of this call: every input check has run by now
                 if prof: prof.mark("prefill + first token")
                 return speculative
 
@@ -660,12 +688,13 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
                 raise ValueError(last_error())
 
             if streamer is not None:
-                streamer.put(prompt.cpu())
+                streamer.put(rows_out.cpu())
             pad = pad_token_id if pad_token_id is not None else (next(iter(eos_ids)) if eos_ids else 0)
-            new_tokens = _stream_decode(engine, kv, None, sampling, B, max_new_tokens, eos_ids, pad, prompt,
+            new_tokens = _stream_decode(engine, kv, None, sampling, N, max_new_tokens, eos_ids, pad, rows_out,
                                         streamer, stopping_criteria,
                                         run_ahead=int(getattr(self.config, "b2_run_ahead", 8)), begun=True,
-                                        lookup_steps=_LOOKUP_STEPS_IN_FLIGHT if began_lookup[0] else 0)
+                                        lookup_steps=_LOOKUP_STEPS_IN_FLIGHT if began_lookup[0] else 0,
+                                        slot_of_row=None if fork is None else fork.slot_of_row)
             engine.check_async_error()
             if prof: prof.mark("decode")
             if plan is not None:
@@ -675,11 +704,14 @@ class LlavaLlamaForCausalLM(nn.Module, LlavaMetaForCausalLM):
             self._pool.release(kv, record)
         if streamer is not None:
             streamer.end()
-        out = torch.cat([prompt, new_tokens.to(device=prompt.device, dtype=prompt.dtype)], dim=1)
+        out = torch.cat([rows_out, new_tokens.to(device=prompt.device, dtype=prompt.dtype)], dim=1)
         if prof: prof.mark("ids to caller"); prof.report()
         if not want:
             return out
         n = new_tokens.shape[1]
+        if fork is not None:  # slot order -> HF row order
+            order = torch.tensor(fork.slot_of_row, device=engine.device)
+            rows = {k: None if v is None else v.index_select(1, order) for k, v in rows.items()}
         return _decoder_output(out, _trim_steps(rows.pop("scores"), n), _trim_steps(rows.pop("logits"), n))
 
     def compute_transition_scores(self, sequences, scores, beam_indices=None, normalize_logits=False):
@@ -1118,6 +1150,31 @@ def _output_arguments(return_dict_in_generate, output_scores, output_logits, kwa
     return {"scores": bool(output_scores), "logits": bool(output_logits)}
 
 
+def _num_return_arguments(config, kwargs, B, do_sample, images):
+    """generate(num_return_sequences=n) without beams: takes n out of `kwargs` and checks what the fork does not serve. Greedy
+    raises transformers' GenerationConfig.validate error; do_sample with temperature <= 1e-5 decodes greedily and returns n
+    equal rows."""
+    n = kwargs.pop("num_return_sequences", None)
+    n = 1 if n is None else int(n)
+    if n == 1:
+        return 1
+    if n < 1:
+        raise ValueError(f"num_return_sequences must be a positive integer, got {n}")
+    if not do_sample:
+        from transformers import GenerationConfig
+
+        GenerationConfig(num_return_sequences=n).validate()
+    if kwargs.get("prompt_lookup_num_tokens") is not None:
+        raise ValueError(f"num_return_sequences has to be 1 when doing assisted generate, but is {n}.")
+    if images is not None and not torch.is_tensor(images):
+        raise NotImplementedError("num_return_sequences > 1 with a list of images: transformers does not expand a list to the "
+                                  "samples of each prompt; pass the images as one tensor")
+    if B == 1 and int(getattr(config, "b2_continuous_batching", 0) or 0) >= 2:
+        raise NotImplementedError("num_return_sequences > 1 together with the continuous batcher (b2_continuous_batching) is "
+                                  "not implemented")
+    return n
+
+
 def _trim_steps(buf, n):
     """generate()'s rows [max_new_tokens, rows, V] -> a tuple of the first n steps' [rows, V] tensors. The decode steps were
     ordered before later work on the caller's current stream when they were queued, so reading there is safe; a buffer with
@@ -1142,7 +1199,7 @@ _LOOKUP_STEPS_IN_FLIGHT = 2
 
 
 def _stream_decode(engine, kv, logits, sampling, B, max_new_tokens, eos_ids, pad, prompt, streamer, stopping_criteria,
-                   run_ahead=8, begun=False, lookup_steps=0):
+                   run_ahead=8, begun=False, lookup_steps=0, slot_of_row=None):
     """Host half of the decode loop. The device chooses token 0 from the prefill `logits` and then runs up to `run_ahead`
     steps in front of this loop; `engine.stream_wait(kv, t, B)` hands over token t as soon as its kernel has written it
     to pinned memory. Per token, in the order HF's loop uses: finished rows show `pad`; streamer.put; eos bookkeeping;
@@ -1150,7 +1207,9 @@ def _stream_decode(engine, kv, logits, sampling, B, max_new_tokens, eos_ids, pad
     tensor, llava/mm_utils.py:92-114). Returns a CPU int64 tensor [B, n], 1 <= n <= max_new_tokens.
     lookup_steps > 0 (a prompt-lookup generation): a step publishes a varying number of tokens, so instead of counting tokens the
     loop asks the engine before each token to keep `lookup_steps` verify steps in flight (b2_stream_enqueue tops them up against
-    the steps the device has retired and queues none once max_new_tokens are published)."""
+    the steps the device has retired and queues none once max_new_tokens are published).
+    slot_of_row (a forked generation, llava/_b2/fork.py): row r of the result, of the streamer and of the criteria is the device's
+    slot slot_of_row[r]."""
     Lt = prompt.shape[1]
     crit_buf = None
     if stopping_criteria:
@@ -1172,6 +1231,8 @@ def _stream_decode(engine, kv, logits, sampling, B, max_new_tokens, eos_ids, pad
                 engine.stream_enqueue(kv, n)
                 scheduled += n
         toks = engine.stream_wait(kv, t, B)
+        if slot_of_row is not None:
+            toks = [toks[s] for s in slot_of_row]
         col = [pad if finished[b] else int(toks[b]) for b in range(B)]
         cols.append(col)
         if streamer is not None:
